@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- FasterSeg student (arch_1, F12.L16) inference FPS @ 1x3x1024x2048 on N B200s.
+"""bench.py -- FasterSeg student (arch_1, F12.L16) inference FPS @ 1x3x1024x2048 on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one 1024x2048 frame through the student network (BASELINE.json configs[1]).
@@ -12,14 +12,17 @@ One "step" = one 1024x2048 frame through the student network (BASELINE.json conf
           (tools/engine/evaluator.py:206-225): pinned-host uint8 HWC image -> H2D -> normalisation folded into the stem kernel
           -> network -> fused upsample+argmax -> uint8 label map D2H, 3 frames in flight.  `e2e_fp32_input` is the same with
           the normalised fp32 NCHW frame of round 1 (25 MB per frame over PCIe).
-  roofline    : the dominant kernel (tcgen05 implicit-GEMM conv) timed live on BOTH 9.66-GFLOP layers of the frame
+  roofline    : the dominant kernel (wgmma implicit-GEMM conv) timed live on BOTH 9.66-GFLOP layers of the frame
                 (heads8 3x3 128->128 @128x256 and stem.1.conv2 64->64 @256x512); the line reports the WORSE of the two
   supernet_steps: the other half of BASELINE's metric -- pretrain (configs[2]) and search (configs[4]) step of the 16-layer
                 supernet with the reference's OHEM criterion, as captured passes; under torchrun data parallel (SyncBN over
                 NVLink peer memory + one flat gradient all-reduce), images/s summed over ranks
   cpu_baseline: the CPU oracle port of the reference path (same weights) on the host cores (N=1, rank 0 only)
 Multi-GPU: inference has no exchange step -> N independent replicas ("replicas only"), weak scaling.
-`--impl reference` times the reference's CPU path (oracle port; the Python reference tree does not exist on the GPU box).
+`--impl reference` times the reference's CPU path (the reference itself where oracle/ref_harness.py finds it, else the oracle port).
+`--dump-outputs DIR` writes, after the timed steps, the logits of the last timed frame as DIR/logits.npy (float32, every second row
+and column of the 1x19x1024x2048 output: 1x19x512x1024, 40 MB); inputs and weights are seeded, so two builds can be compared
+output for output.
 """
 import argparse
 import json
@@ -71,7 +74,7 @@ def synth_weights_(model, seed=12345):
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled every 100 ms during the timed regions (B200_PROFILING.md).  Uses NVML in-process
+    """SM clock / throttle reasons sampled every 100 ms during the timed regions.  Uses NVML in-process
     (nvidia_ml_py): spawning `nvidia-smi -lms` next to a host-driven copy/launch pipeline halves its throughput because each
     poll takes driver locks; the nvidia-smi CLI is only the fallback."""
 
@@ -148,12 +151,11 @@ def measured_peaks():
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d["bf16_tflops"], "tflops_sustained": d.get("bf16_tflops_sustained"),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "tflops": 1590.0, "tflops_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16/BF16 -- not measured
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "tflops_sustained": None, "source": "datasheet"}
 
 
-KERNEL_NAMES = {0: "conv_direct_kernel", 1: "conv_tc_kernel (per-tap, 128 px x Cout tile)", 2: "conv_tc2_kernel (row strip)",
-                3: "conv_tc3_kernel (channel-major 128 x 256 MMA)", 4: "conv_tc4_kernel (CTA pair, cta_group::2)",
-                5: "conv_tc5_kernel (tap-concatenated N = 3*Cout, flattened-pixel tiles)"}
+KERNEL_NAMES = {0: "conv_direct_kernel", 1: "conv_tc_kernel (wgmma, 128 px x N tile)", 2: "conv_tc_kernel (wgmma, row strip: one input window per chunk)"}
 
 
 def _time_conv_layer(device, Cin, Cout, h, w, reps=5):
@@ -162,7 +164,7 @@ def _time_conv_layer(device, Cin, Cout, h, w, reps=5):
     from fasterseg_b200 import _lib
     from fasterseg_b200 import functional as F_
     per_pair = 2.0 * (Cin + Cout) * h * w
-    nbuf = max(6, int(160e6 / per_pair) + 1)   # > 126 MB L2: every launch reads its input from HBM
+    nbuf = max(6, int(160e6 / per_pair) + 1)   # > 50 MB L2: every launch reads its input from HBM
     xs = [F_.empty_nhwc(1, Cin, h, w, device).normal_() for _ in range(nbuf)]
     ys = [F_.empty_nhwc(1, Cout, h, w, device) for _ in range(nbuf)]
     wt = torch.randn(Cout, Cin, 3, 3, device=device) * 0.03
@@ -185,17 +187,12 @@ def _time_conv_layer(device, Cin, Cout, h, w, reps=5):
 
 
 def dominant_kernel_roofline(device):
-    """The tcgen05 implicit-GEMM conv on the two most expensive launches of the student frame (9.66 GFLOP each, 17 % of the
+    """The wgmma implicit-GEMM conv on the two most expensive launches of the student frame (9.66 GFLOP each, 17 % of the
     frame's FLOPs each): heads8.conv_3x3 (128 -> 128 channels on the 128x256 map, intensity 566 FLOP/B: tensor-bound) and
     stem.1.conv2 (64 -> 64 on the 256x512 map, intensity 288 FLOP/B: at the ridge, 5.7 us by FLOPs vs 5.1 us by bytes).
     Algorithmic work per launch: 2*9*Cin*Cout*h*w FLOP; bytes = input + output + weights, each once, fp16.
     The line's `roofline` is the WORSE of the two; both are listed under `layers`."""
     pk = measured_peaks()
-    traffic = {}  # dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` captures, per layer
-    tj = os.path.join(ROOT, "profiles", "r2_roofline_traffic.json")
-    if os.path.isfile(tj):
-        with open(tj) as f:
-            traffic = {k: v.get("traffic_bytes") for k, v in json.load(f).get("layers", {}).items()}
     layers = []
     for label, Cin, Cout, h, w in (("heads8.conv_3x3: 3x3 128->128 @128x256", 128, 128, 128, 256),
                                    ("stem.1.conv2: 3x3 64->64 @256x512", 64, 64, 256, 512)):
@@ -211,12 +208,8 @@ def dominant_kernel_roofline(device):
                        "us_per_launch": round(us, 2), "roofline_us": round(max(t_tensor, t_hbm) * 1e6, 2),
                        "algorithmic_flops": flops, "algorithmic_bytes": abytes})
     worst = dict(min(layers, key=lambda r: r["frac"]))
-    worst.update({"traffic": next((v for k, v in traffic.items() if k in worst["kernel"]), None), "peak_source": pk["source"], "layers": layers,
-                  "note": "worse of the two 9.66-GFLOP launches of the frame.  A tcgen05.mma costs ~130-180 cycles whatever N is "
-                          "(tools/umma_rate.cu), so heads8 runs channel-major (weights as M = 128, 256 pixels as N) and "
-                          "stem.1.conv2 (64 output channels) concatenates the three horizontal taps along N (N = 192, 12 MMAs per "
-                          "120 pixels instead of 36 per 128) and applies the horizontal shift in the epilogue; with K = 576 the "
-                          "accumulator drain (TMEM -> registers, 98 KB per tile) is as long as the MMAs themselves"})
+    worst.update({"peak_source": pk["source"], "layers": layers,
+                  "note": "worse of the two 9.66-GFLOP launches of the frame"})
     return worst
 
 
@@ -538,13 +531,18 @@ def main():
     ap.add_argument("--warmup", type=int, default=20)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the logits of the last timed frame (float32, every second row and column) to DIR/logits.npy")
     ap.add_argument("--no-supernet-step", action="store_true",
                     help="skip the secondary metrics (supernet pretrain / search step, BASELINE configs[2] / [4]; distillation "
                          "step, configs[3])")
     args = ap.parse_args()
     if args.impl == "reference":
+        # a CPU sample: a frame costs ~0.2-1 s of CPU time, so the arm refuses long runs instead of shortening them
         if args.steps > 30:
-            args.steps = 30  # bounded CPU sample (a frame costs ~0.2-1 s of CPU time)
+            ap.error("--impl reference times at most 30 steps (got --steps %d)" % args.steps)
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes what the GPU path computed; it is not available with --impl reference")
         return run_reference(args)
     args.warmup = max(args.warmup, 3)
 
@@ -571,7 +569,7 @@ def main():
 
     # ---- device-resident FPS (value) ----
     g = torch.Generator(device="cpu").manual_seed(12345 + rank)
-    npool = 6  # 6 x 25.2 MB = 151 MB of distinct frames > 126 MB L2
+    npool = 6  # 6 x 25.2 MB = 151 MB of distinct frames > 50 MB L2
     pool = [torch.randn(1, 3, H, W, generator=g).to(device) for _ in range(npool)]
     runner = GraphedInference(model, pool[0], mode="logits", logits_dtype=torch.float16)
     launches_value = runner.launches_per_replay
@@ -585,12 +583,18 @@ def main():
         dist.barrier()
     torch.cuda.synchronize()
     st, en = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    out = None
     st.record()
     for i in range(args.steps):
-        runner(pool[i % npool])
+        out = runner(pool[i % npool])
     en.record()
     torch.cuda.synchronize()
     ms_total = st.elapsed_time(en)
+    if args.dump_outputs and rank == 0 and out is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), out[:, :, ::2, ::2].float().cpu().numpy())
+    del out
     if world > 1:
         t = torch.tensor([ms_total], device=device)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -662,7 +666,7 @@ def main():
         "config": {"workload": WORKLOAD,
                    "arithmetic": "fp16 NHWC storage / fp32 accumulate, full-res fp16 logits materialised",
                    "parallelism": "replicas x%d (no exchange step in inference)" % world,
-                   "l2_policy": "inputs rotate through a 6-frame device pool (151 MB > 126 MB L2); activations per frame "
+                   "l2_policy": "inputs rotate through a 6-frame device pool (151 MB > 50 MB L2); activations per frame "
                                 "(~430 MB) exceed L2",
                    "timing": "CUDA events around %d CUDA-graph replays, max over ranks" % args.steps,
                    "frame_gflop": STUDENT_GFLOP},

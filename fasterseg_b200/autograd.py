@@ -1,4 +1,4 @@
-"""torch.autograd.Function wrappers: the training-mode forward/backward of the hot path on the sm_100a kernels.
+"""torch.autograd.Function wrappers: the training-mode forward/backward of the hot path on the sm_90a kernels.
 
 The reference gets its backward from autograd over F.conv2d / BatchNorm2d / ReLU / F.interpolate / torch.cat and the
 `result + op(x) * w` python arithmetic (search/operations.py, search/model_search.py:60-78,318-333).  Here each fused unit

@@ -1,4 +1,4 @@
-"""Build libfsb200.so (sm_100a) in-tree with nvcc.  Used by __graft_entry__.build() and `python -m fasterseg_b200.build`."""
+"""Build libfsb200.so (sm_90a) in-tree with nvcc.  Used by __graft_entry__.build() and `python -m fasterseg_b200.build`."""
 import os
 import subprocess
 import sys
@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfsb200.so")
-SOURCES = ["api.cu", "conv_tc.cu", "conv_tc2.cu", "conv_tc3.cu", "conv_tc4.cu", "conv_tc5.cu", "conv_direct.cu", "resize.cu", "bn.cu", "train.cu", "wgrad_tc.cu", "train_fused.cu", "loss.cu", "optim.cu", "dp.cu", "peer.cu"]
+SOURCES = ["api.cu", "conv_tc.cu", "conv_direct.cu", "resize.cu", "bn.cu", "train.cu", "wgrad_tc.cu", "train_fused.cu", "loss.cu", "optim.cu", "dp.cu", "peer.cu"]
 HEADERS = ["fsb_common.cuh", "fsb_internal.h", os.path.join("..", "..", "include", "fsb200.h")]
 
 
@@ -25,7 +25,7 @@ def build(force=False, verbose=False):
     if not force and not needs_build():
         return LIB
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
            "-shared", "-Xcompiler", "-fPIC", "-o", LIB] + SOURCES + ["-ldl"]
     if verbose:
         cmd.insert(1, "-Xptxas")

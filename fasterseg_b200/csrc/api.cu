@@ -33,7 +33,7 @@ int sm_count() {
   if (n == 0) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
   }
   return n;
 }
@@ -111,7 +111,6 @@ int stat_rows(int64_t);
 int wsum_rows(int64_t, int);
 int rowsum_launch(int, const float*, int, int, float*, cudaStream_t);
 int conv_tc_m_tiles(const fsb_conv_desc*);
-int conv_tc2_ctas(const fsb_conv_desc*);
 int bn_finalize_launch(int, const float*, int, int, double, const float*, const float*, float, float, float*, float*, float*, float*,
                        float*, float*, cudaStream_t, long long* = nullptr, const fsb_bn_sel* = nullptr, const int* = nullptr, int = 0);
 int affine_act_launch(int64_t, int, const void*, int, const float*, const float*, void*, int, uint32_t, cudaStream_t,
@@ -145,7 +144,8 @@ int wsum_bwd_launch(int, int64_t, int, const void*, int, const void* const*, con
                     float*, float, cudaStream_t);
 int add_inplace_launch(int64_t, int, const void*, int, void*, int, cudaStream_t);
 
-extern unsigned long long* g_dbg_buffer;
+// device buffer for in-kernel timelines of experimental kernels (fsb_debug_set_buffer); no kernel of this build writes it
+unsigned long long* g_dbg_buffer = nullptr;
 
 static int check_desc(const fsb_conv_desc* d) {
   if (!d) return set_error(FSB_ERR_INVALID, "null conv desc");
@@ -201,17 +201,14 @@ int fsb_get_option(const char* name) {
 int fsb_conv_stats_rows(const fsb_conv_desc* d) {
   if (check_desc(d)) return 0;
   if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d)) return stat_rows(static_cast<int64_t>(d->N) * d->Ho * d->Wo);
-  if (conv_tc2_supported(d)) return conv_tc2_ctas(d);
   return conv_tc_m_tiles(d);
 }
 int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats) {
   if (check_desc(d)) return -1;
   if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d)) return 0;
-  if (!with_stats && conv_tc5_supported(d, y)) return 5;
-  if (!with_stats && conv_tc4_supported(d, y)) return 4;
-  if (!with_stats && conv_tc3_supported(d, y)) return 3;
-  if (conv_tc2_supported(d)) return 2;
-  return 1;
+  (void)y;
+  (void)with_stats;
+  return conv_tc_strip(d) ? 2 : 1;
 }
 int fsb_stat_rows(int64_t pixels) { return stat_rows(pixels); }
 int fsb_wsum_rows(int64_t pixels, int C) { return wsum_rows(pixels, C); }
@@ -295,7 +292,7 @@ int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, con
   if (!x || !wpacked || !y) return set_error(FSB_ERR_INVALID, "conv_fwd: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d)) return conv_direct_launch(d, x, wpacked, scale, shift, y, stats, st);
-  return conv_tc_dispatch(d, x, wpacked, scale, shift, y, stats, st);
+  return conv_tc_launch(d, x, wpacked, scale, shift, y, stats, st);
 }
 
 int fsb_stem_conv_nchw(int N, int H, int W, int Cout, const void* x, int x_is_f32, const float* w, const float* scale,

@@ -51,7 +51,7 @@ __host__ __device__ __forceinline__ int split_remap(int c, int h, int hmax) {
 int stat_rows(int64_t pixels) {
   int64_t b = (pixels + 255) / 256;
   if (b < 1) b = 1;
-  if (b > 148 * 2) b = 148 * 2;
+  if (b > 132 * 2) b = 132 * 2;
   return static_cast<int>(b);
 }
 
@@ -333,7 +333,7 @@ int affine_act_launch(int64_t pixels, int C, const void* x, int xcs, const float
     return set_error(FSB_ERR_INVALID, "affine_act: C/strides multiples of 8, pointers 16B aligned");
   const int64_t total = pixels * (C / 8);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   if (flags & FSB_ACT_IN_F32)
     FSB_LAUNCH(affine_act_kernel<float>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, pixels, C / 8,

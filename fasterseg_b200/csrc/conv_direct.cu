@@ -1,5 +1,5 @@
 // conv_direct.cu -- CUDA-core convolution kernels + weight packing.
-//   * pack_conv_weight_kernel : fp32 OIHW (max-width, sliced) -> fp16 [tap][Npad][Kpad] for the tcgen05 kernel
+//   * pack_conv_weight_kernel : fp32 OIHW (max-width, sliced) -> fp16 [tap][Npad][Kpad] for the tensor-core kernels
 //   * conv_direct_kernel      : generic NHWC fp16 direct conv on the same packed weights (Cin < 16, odd strides of
 //                               the API, and the device-side cross-check of the tensor-core kernel in tests)
 //   * stem_conv_nchw_kernel   : 3x3 s2 p1 RGB stem reading the caller's NCHW fp32/fp16 tensor directly, so the
@@ -35,7 +35,7 @@ int pack_conv_weight(const fsb_conv_desc* d, const float* w, int64_t so, int64_t
   const ConvGeom g = conv_geom(d);
   const int64_t total = static_cast<int64_t>(g.taps) * g.npad * g.kpad;
   int blocks = static_cast<int>((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   FSB_LAUNCH(pack_conv_weight_kernel, dim3(blocks), dim3(256), 0, stream, w, so, si, g.taps, d->Cout, d->Cin, g.npad, g.kpad,
                                                       static_cast<__half*>(packed));
   cudaError_t e = last_launch_error();
@@ -227,48 +227,41 @@ stem_conv_nchw_kernel(int N, int H, int W, int Cout, const TIn* __restrict__ x, 
 // RGB stem on the tensor cores: a CTA (128 threads) owns 128 consecutive output pixels of one output row.  Thread t
 // gathers the 27 inputs of its pixel straight from the NCHW tensor (warp-coalesced per (channel,row)), converts to
 // fp16 and writes row t of a 128 x 32 K-major A tile in the SWIZZLE_64B canonical layout (K = 27 padded to 32); the
-// OIHW weights are laid out the same way as the B tile.  Two tcgen05.mma (K = 16 each) produce the 128 x Cout fp32
-// tile in TMEM; the epilogue applies BN scale/shift + ReLU and each thread stores its pixel's Cout fp16 values
-// contiguously (a warp writes 32 x 2*Cout contiguous bytes).  No im2col buffer, no fp16 NHWC copy of the image.
+// OIHW weights are laid out the same way as the B tile.  The CTA is one warpgroup: four wgmma (two m64 halves x K = 16 each)
+// produce the 128 x NP fp32 tile in registers, parked in shared memory as [channel][pixel]; the epilogue applies BN
+// scale/shift + ReLU and each thread stores its pixel's Cout fp16 values contiguously (a warp writes 32 x 2*Cout contiguous
+// bytes).  No im2col buffer, no fp16 NHWC copy of the image.
 // ------------------------------------------------------------------------------------------
 // TIn = uint8_t: the frame is the camera / dataset image itself, uint8 HWC (tools/engine/evaluator.py:206-225 hands the model
 // `normalize(img, mean, std)` = (img / 255 - mean) / std as fp32 CHW, evaluator.py:329, tools/utils/img_utils.py:179-185).  The
 // normalisation is a 3 x 256 lookup table of fp16 values (exactly the fp16 rounding of what the reference computes for each
 // byte value), so the H2D copy shrinks 4x and the result is bit-identical to feeding the normalised fp32 image.
-template <typename TIn>
+constexpr int kStemAccLd = 128 + 4;  // padded channel column of the parked accumulator (conflict-free stores and reads)
+
+template <typename TIn, int NP>  // NP: wgmma N, Cout rounded up to 32 or 64
 __global__ void __launch_bounds__(128)
 stem_conv_tc_kernel(int N, int H, int W, int Cout, int npad, const TIn* __restrict__ x, const float* __restrict__ w,
                     const float* __restrict__ scale, const float* __restrict__ shift, __half* __restrict__ y,
-                    int y_cstride, uint32_t flags, uint32_t tmem_cols, const __half* __restrict__ lut) {
+                    int y_cstride, uint32_t flags, const __half* __restrict__ lut) {
   __shared__ __align__(1024) uint8_t s_a[128 * 64];
   __shared__ __half s_lut[std::is_same<TIn, uint8_t>::value ? 768 : 2];
   __shared__ __align__(1024) uint8_t s_b[64 * 64];
-  __shared__ __align__(8) uint64_t s_bar;
-  __shared__ uint32_t s_tmem;
   __shared__ float s_scale[64];
   __shared__ float s_shift[64];
+  __shared__ float s_acc[NP * kStemAccLd];
   pdl_launch_dependents();
   const int t = threadIdx.x;
-  const int warp = t >> 5;
   const int Ho = H / 2 + (H & 1), Wo = W / 2 + (W & 1);
   const int wo = blockIdx.x * 128 + t;
   const int ho = blockIdx.y;
   const int n = blockIdx.z;
-  if (t == 0) {
-    mbar_init(&s_bar, 1);
-    mbar_fence_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(&s_tmem, tmem_cols);
-    tmem_relinquish();
-  }
   pdl_wait();  // weights / scale / shift may have been produced by the immediately preceding kernel
   if constexpr (std::is_same<TIn, uint8_t>::value) {
     for (int i = t; i < 768; i += 128) s_lut[i] = lut[i];
     __syncthreads();
   }
-  // weights -> B tile rows (one thread per output channel), fp32 OIHW is already [co][27]
-  if (t < npad) {
+  // weights -> B tile rows (one thread per output channel, zero rows up to NP), fp32 OIHW is already [co][27]
+  if (t < NP) {
     __half hv[32];
 #pragma unroll
     for (int k = 0; k < 32; ++k) hv[k] = __float2half_rn((t < Cout && k < 27) ? w[t * 27 + k] : 0.f);
@@ -313,34 +306,37 @@ stem_conv_tc_kernel(int N, int H, int W, int Cout, int npad, const TIn* __restri
       *reinterpret_cast<uint4*>(s_a + t * 64 + ((j ^ ((t >> 1) & 3)) << 4)) = *reinterpret_cast<const uint4*>(&hv[j * 8]);
   }
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy smem writes -> visible to the MMA (async proxy)
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = s_tmem;
-  if (t < 32) {   // converged warp 0, elected lane issues (uniform operands: no per-instruction waterfall)
-    const uint32_t idesc = umma_idesc_f16(128, static_cast<uint32_t>(npad));
-    const uint64_t da = umma_desc_kmajor(smem_u32(s_a), 64);
-    const uint64_t db = umma_desc_kmajor(smem_u32(s_b), 64);
-    if (elect_one()) {
-      umma_f16_ss(tmem, da, db, idesc, 0u);
-      umma_f16_ss(tmem, da + 2, db + 2, idesc, 1u);
-      umma_commit(&s_bar);
+  {
+    float acc[2][NP / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NP / 2; ++i) acc[h][i] = 0.f;
+    const uint64_t da = wgmma_desc_kmajor(smem_u32(s_a), 64);
+    const uint64_t db = wgmma_desc_kmajor(smem_u32(s_b), 64);
+    constexpr uint64_t kHalf = (64 * 64) >> 4;  // pixel rows 64..127 of the A tile
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {  // K = 32 = two steps of 16 fp16 (32 B, +2 in the address field)
+      wgmma_f16<NP, 0>(acc[0], da + 2 * k, db + 2 * k);
+      wgmma_f16<NP, 0>(acc[1], da + kHalf + 2 * k, db + 2 * k);
     }
-    __syncwarp();
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NP / 2; ++i) s_acc[wgmma_col(t, i) * kStemAccLd + 64 * h + wgmma_row(t, i)] = acc[h][i];
   }
-  mbar_wait(&s_bar, 0);
-  tc_fence_after();
+  __syncthreads();
   const bool relu = flags & FSB_CONV_RELU;
   __half* yp = y + (static_cast<size_t>(n) * Ho * Wo + static_cast<size_t>(ho) * Wo + wo) * y_cstride;
-  const uint32_t taddr = tmem + (static_cast<uint32_t>(warp * 32) << 16);
   for (int c = 0; c < npad; c += 16) {
-    uint32_t v[16];
-    tmem_ld16(taddr + c, v);
-    tmem_ld_wait();
     float f[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
-      const float a = __uint_as_float(v[j]) * s_scale[c + j] + s_shift[c + j];
+      const float a = s_acc[(c + j) * kStemAccLd + t] * s_scale[c + j] + s_shift[c + j];
       f[j] = relu ? fmaxf(a, 0.f) : a;
     }
     if (wo < Wo) {
@@ -364,12 +360,6 @@ stem_conv_tc_kernel(int N, int H, int W, int Cout, int npad, const TIn* __restri
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, tmem_cols);
-  }
 }
 
 int stem_conv_nchw_launch(int N, int H, int W, int Cout, const void* x, int x_is_f32, const float* w, const float* scale,
@@ -378,13 +368,22 @@ int stem_conv_nchw_launch(int N, int H, int W, int Cout, const void* x, int x_is
   const int cpad = (Cout + 15) / 16 * 16;
   if (cpad <= 64 && !(flags & FSB_CONV_FORCE_DIRECT)) {
     dim3 grid_tc((Wo + 127) / 128, Ho, N);
-    const uint32_t cols = cpad <= 32 ? 32u : 64u;
-    if (x_is_f32)
-      FSB_LAUNCH(stem_conv_tc_kernel<float>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, static_cast<const float*>(x), w,
-                 scale, shift, static_cast<__half*>(y), y_cstride, flags, cols, static_cast<const __half*>(nullptr));
-    else
-      FSB_LAUNCH(stem_conv_tc_kernel<__half>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, static_cast<const __half*>(x), w,
-                 scale, shift, static_cast<__half*>(y), y_cstride, flags, cols, static_cast<const __half*>(nullptr));
+    const __half* no_lut = nullptr;
+    if (x_is_f32) {
+      if (cpad <= 32)
+        FSB_LAUNCH(stem_conv_tc_kernel<float, 32>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, static_cast<const float*>(x), w,
+                   scale, shift, static_cast<__half*>(y), y_cstride, flags, no_lut);
+      else
+        FSB_LAUNCH(stem_conv_tc_kernel<float, 64>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, static_cast<const float*>(x), w,
+                   scale, shift, static_cast<__half*>(y), y_cstride, flags, no_lut);
+    } else {
+      if (cpad <= 32)
+        FSB_LAUNCH(stem_conv_tc_kernel<__half, 32>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, static_cast<const __half*>(x),
+                   w, scale, shift, static_cast<__half*>(y), y_cstride, flags, no_lut);
+      else
+        FSB_LAUNCH(stem_conv_tc_kernel<__half, 64>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, static_cast<const __half*>(x),
+                   w, scale, shift, static_cast<__half*>(y), y_cstride, flags, no_lut);
+    }
     cudaError_t e2 = last_launch_error();
     if (e2 != cudaSuccess) return set_cuda_error(e2, "stem_conv_tc launch");
     return FSB_OK;
@@ -410,9 +409,12 @@ int stem_conv_u8hwc_launch(int N, int H, int W, int Cout, const uint8_t* x, cons
   const int cpad = (Cout + 15) / 16 * 16;
   if (cpad > 64) return set_error(FSB_ERR_UNSUPPORTED, "stem_conv_u8hwc: Cout <= 64");
   dim3 grid_tc((Wo + 127) / 128, Ho, N);
-  const uint32_t cols = cpad <= 32 ? 32u : 64u;
-  FSB_LAUNCH(stem_conv_tc_kernel<uint8_t>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, x, w, scale, shift,
-             static_cast<__half*>(y), y_cstride, flags, cols, static_cast<const __half*>(lut));
+  if (cpad <= 32)
+    FSB_LAUNCH(stem_conv_tc_kernel<uint8_t, 32>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, x, w, scale, shift,
+               static_cast<__half*>(y), y_cstride, flags, static_cast<const __half*>(lut));
+  else
+    FSB_LAUNCH(stem_conv_tc_kernel<uint8_t, 64>, grid_tc, dim3(128), 0, stream, N, H, W, Cout, cpad, x, w, scale, shift,
+               static_cast<__half*>(y), y_cstride, flags, static_cast<const __half*>(lut));
   cudaError_t e = last_launch_error();
   if (e != cudaSuccess) return set_cuda_error(e, "stem_conv_u8hwc launch");
   return FSB_OK;
@@ -448,7 +450,7 @@ int confusion_launch(int64_t n, const uint8_t* pred, const void* gt, int gt_byte
   if (n_cl < 1 || n_cl > 64) return set_error(FSB_ERR_INVALID, "confusion_matrix: 1 <= n_cl <= 64");
   int64_t blocks = (n + 256 * 16 - 1) / (256 * 16);
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   const size_t smem = static_cast<size_t>(n_cl * n_cl + 2) * sizeof(unsigned int);
   unsigned long long* o = reinterpret_cast<unsigned long long*>(out);
   if (gt_bytes == 1)

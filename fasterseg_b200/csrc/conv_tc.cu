@@ -1,4 +1,4 @@
-// conv_tc.cu -- K1: im2col-free implicit-GEMM convolution on tcgen05 tensor cores (sm_100a).
+// conv_tc.cu -- K1: im2col-free implicit-GEMM convolution on Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces F.conv2d (+ BatchNorm eval + ReLU) for every 3x3 / 1x1 conv of the FasterSeg hot path
 // (reference call sites: search/slimmable_ops.py:47, search/operations.py:72-83,146-150,..., search/seg_oprs.py:21-39).
@@ -9,11 +9,13 @@
 //             tap-shifted coordinate; out-of-image rows/cols and channel tails are zero-filled by TMA, so
 //             padding costs nothing and no im2col buffer exists.  Stride-2 convs address one of four
 //             parity planes of the input (each its own tensor map), which keeps every box dense.
-//   B tile  : packed fp16 weights [tap][Npad][Kpad] (K-major), one TMA box {BK, Ntile, 1}.
-//   D       : fp32 accumulator in TMEM (128 lanes x Ntile columns).
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + single-thread MMA issuer,
-// warps 2-5 = epilogue (tcgen05.ld -> BN scale/shift -> ReLU -> fp16 -> NHWC store with channel offset/stride,
-// which is how torch.cat(dim=1) call sites become free).
+//   B tile  : packed fp16 weights [tap][Npad][Kpad] (K-major), one TMA box {BK, NT, 1}.
+//   D       : fp32 accumulator in the registers of one warpgroup (two m64 halves of the 128-pixel tile, NT <= 128
+//             columns each: at most 128 accumulator registers per thread).
+// Warp roles (256 threads): warp 0 = TMA producer (warps 1-3 only join the final barrier), warps 4-7 = the MMA warpgroup.
+// After the main loop the warpgroup parks the accumulator in shared memory as [channel][pixel] and runs the epilogue on it
+// (BN scale/shift -> ReLU -> fp16 -> NHWC store with channel offset/stride, which is how torch.cat(dim=1) call sites
+// become free), one pixel per thread.
 #include "fsb_common.cuh"
 #include "fsb_internal.h"
 
@@ -21,7 +23,8 @@ namespace fsb {
 
 constexpr int kTileM = 128;
 constexpr int kMaxStages = 8;
-constexpr int kThreads = 192;
+constexpr int kThreads = 256;
+constexpr int kAccLd = kTileM + 4;  // padded channel column of the parked accumulator: conflict-free fragment stores and row reads
 
 struct ConvTcParams {
   CUtensorMap tmap_a[4];
@@ -39,40 +42,50 @@ struct ConvTcParams {
   int tiles_w, tiles_h;
   int tw, th;
   int Cout;
-  int n_tile;
   int stages;
   int y_cstride;
   uint32_t flags;
-  uint32_t tmem_cols;
   const float* scale;
   const float* shift;
   __half* y;
   float* stats;   // partial rows (one per spatial tile = blockIdx.x), see bn.cu "Deterministic statistics"
   int stats_C;    // row half-width (row stride = 2 * stats_C floats)
   int stats_off;  // channel offset of this conv's output inside a row
-  int ksplit;     // 1, or 3: a cluster of 3 CTAs (blockIdx.z) shares one output tile, CTA z accumulates kernel row z (3 of the 9 taps)
-  uint32_t part_off;  // byte offset (from the 1024-aligned smem base) of the (ksplit - 1) partial-sum buffers [n_tile][128] fp32 in CTA 0
-  int m_tiles;  // persistent kernel only: spatial tiles (tiles_w * tiles_h * N) ...
-  int n_tiles;  // ... x output-channel tiles; a CTA walks tile = blockIdx.x, += gridDim.x (n fastest)
 };
 
-template <int BK>
-__global__ void __launch_bounds__(kThreads, 2)   // <= 170 registers: two CTAs per SM (96 KB pipelines) on the large maps
+// shared memory after the main loop: [0, kOutBytes) = statistics partials or the TMA-store staging slabs,
+// [kOutBytes, + NT * kAccLd * 4) = the parked accumulator; both reuse the (then idle) stage ring
+template <int NT>
+__host__ __device__ constexpr uint32_t conv_tc_out_bytes() { return static_cast<uint32_t>((NT + 63) / 64) * kTileM * 128; }
+template <int NT>
+__host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes() { return conv_tc_out_bytes<NT>() + static_cast<uint32_t>(NT) * kAccLd * 4; }
+
+// Row-strip mode (STRIP, 3x3 stride-1 dilation-1 convs with Cin % 64 == 0 on wide maps): a tile is 128 consecutive output
+// pixels of ONE row (tw = 128, th = 1).  Per 64-channel chunk the producer loads the 3 input rows x 130 pixels the tile needs
+// (left/right halo included) ONCE into a window buffer (ring of 2); the operand of tap (r,s) is the same window read through a
+// descriptor whose start address is shifted by r rows and s pixels (TMA and wgmma both apply the 128B swizzle to absolute
+// shared-memory address bits, so a 128B-multiple shift inside the 1024B-aligned window reads back what TMA wrote).  Only the
+// weights stream per (chunk, tap), through the stage ring.  The input is fetched 3x per chunk instead of 9x.
+constexpr uint32_t kWinBytes = 3 * (kTileM + 2) * 128;
+constexpr uint32_t kWinStride = (kWinBytes + 1023) / 1024 * 1024;
+
+template <int BK, int NT, bool STRIP>
+__global__ void __launch_bounds__(kThreads, (NT <= 64 && !STRIP) ? 2 : 1)
 conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float s_scale[256];
-  __shared__ float s_shift[256];
+  __shared__ __align__(8) uint64_t win_full[2];
+  __shared__ __align__(8) uint64_t win_empty[2];
+  __shared__ float s_scale[NT];
+  __shared__ float s_shift[NT];
 
   pdl_launch_dependents();  // let the next kernel's prologue overlap our main loop / tail
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr uint32_t kABytes = kTileM * BK * 2;
-  const uint32_t b_bytes = static_cast<uint32_t>(p.n_tile) * BK * 2;
-  const uint32_t stage_bytes = kABytes + b_bytes;
+  constexpr uint32_t kStageBytes = STRIP ? NT * BK * 2 : kABytes + NT * BK * 2;
+  static_assert(!STRIP || BK == 64, "row-strip windows are 128B-swizzled 64-channel rows");
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   // tile coordinates
@@ -83,100 +96,155 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   const int img = t / p.tiles_h;
   const int w0 = tile_w * p.tw;
   const int h0 = tile_h * p.th;
-  const int n0 = blockIdx.y * p.n_tile;
-  // split-K over a cluster (K1 on small maps): a tcgen05.mma costs ~150 cycles whatever its N (tools/umma_rate.cu), so a tile's
-  // main loop is a serial chain of 9 * Cin / 16 instructions however small the map is.  With ksplit = 3 the three kernel rows
-  // run on three SMs; CTAs 1 and 2 hand their fp32 accumulators to CTA 0 through distributed shared memory.
-  const int kz = p.ksplit > 1 ? static_cast<int>(blockIdx.z) : 0;
-  const int taps_local = p.taps / p.ksplit;
-  const int tap0 = kz * taps_local;
-  const int k_iters = taps_local * p.k_chunks;
+  const int n0 = blockIdx.y * NT;
+  const int k_iters = p.taps * p.k_chunks;
 
   if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&p.tmap_a[0]);
     tma_prefetch_desc(&p.tmap_b);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);  // one arrival per warp of the MMA warpgroup
     }
-    mbar_init(&tmem_full_bar, 1);
+    for (int w = 0; w < 2; ++w) {
+      mbar_init(&win_full[w], 1);
+      mbar_init(&win_empty[w], 4);
+    }
     mbar_fence_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_smem, p.tmem_cols);
-    tmem_relinquish();
   }
   pdl_wait();  // predecessor's outputs (our x) and anything it still reads (our y) are safe from here on
   // epilogue constants
-  for (int c = threadIdx.x; c < p.n_tile; c += kThreads) {
+  for (int c = threadIdx.x; c < NT; c += kThreads) {
     const int ch = n0 + c;
     const bool ok = ch < p.Cout;
     s_scale[c] = (ok && (p.flags & FSB_CONV_AFFINE) && p.scale) ? p.scale[ch] : 1.0f;
     s_shift[c] = (ok && (p.flags & FSB_CONV_AFFINE) && p.shift) ? p.shift[ch] : 0.0f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
 
-  // Issue style (tools/umma_rate.cu): the producer and MMA warps stay CONVERGED and only the TMA / MMA instructions themselves
-  // sit under elect.sync.  Inside an `if (lane == 0)` region the compiler has to wrap every uniform-datapath instruction
-  // (UTMALDG, UTCHMMA, UTCBAR) into an ELECT / R2UR / BRA.U.ANY waterfall, which cost ~130 cycles per MMA in round 1.
-  if (warp == 0) {
-    // ================= TMA producer =================
+  if (STRIP && warp == 0) {
+    // ================= TMA producer, row strip: one input window per chunk, one weight tile per (chunk, tap) =================
+    uint8_t* bring = smem + 2 * kWinStride;
+    RingPos rp, rw;
+    for (int kc = 0; kc < p.k_chunks; ++kc) {
+      mbar_wait_inline(&win_empty[rw.s], rw.phase ^ 1u);
+      if (elect_one()) {
+        mbar_arrive_expect_tx(&win_full[rw.s], kWinBytes);
+        tma_load_4d(smem + rw.s * kWinStride, &p.tmap_a[0], &win_full[rw.s], kc * BK, w0 + p.tap_dw[0], h0 + p.tap_dh[0], img);
+      }
+      __syncwarp();
+      rw.advance(2);
+      for (int tap = 0; tap < 9; ++tap) {
+        mbar_wait_inline(&empty_bar[rp.s], rp.phase ^ 1u);
+        if (elect_one()) {
+          mbar_arrive_expect_tx(&full_bar[rp.s], kStageBytes);
+          tma_load_3d(bring + rp.s * kStageBytes, &p.tmap_b, &full_bar[rp.s], kc * BK, n0, tap);
+        }
+        __syncwarp();
+        rp.advance(p.stages);
+      }
+    }
+  } else if (warp == 0) {
+    // ================= TMA producer (converged warp, one elected lane issues) =================
     RingPos rp;
     uint8_t* sa = smem;
-    for (int tap = tap0; tap < tap0 + taps_local; ++tap) {
+    for (int tap = 0; tap < p.taps; ++tap) {
       const CUtensorMap* ma = &p.tmap_a[p.tap_map[tap]];
       const int cw = w0 + p.tap_dw[tap];
       const int chh = h0 + p.tap_dh[tap];
       const int wi = p.tap_widx[tap];
       for (int kc = 0; kc < p.k_chunks; ++kc) {
-        mbar_wait(&empty_bar[rp.s], rp.phase ^ 1u);
+        mbar_wait_inline(&empty_bar[rp.s], rp.phase ^ 1u);
         if (elect_one()) {
-          mbar_arrive_expect_tx(&full_bar[rp.s], stage_bytes);
+          mbar_arrive_expect_tx(&full_bar[rp.s], kStageBytes);
           tma_load_4d(sa, ma, &full_bar[rp.s], kc * BK, cw, chh, img);
           tma_load_3d(sa + kABytes, &p.tmap_b, &full_bar[rp.s], kc * BK, n0, wi);
         }
         __syncwarp();
-        sa += stage_bytes;
+        sa += kStageBytes;
         rp.advance(p.stages);
         if (rp.s == 0) sa = smem;
       }
     }
-    if (p.ksplit > 1) cluster_sync_all_threads();
-  } else if (warp == 1) {
-    // ================= MMA issuer (converged warp, one elected lane issues) =================
-    // Lean loop: no integer division, descriptors of stage s = descriptors of stage 0 + s * (stage_bytes >> 4) in the
-    // start-address field (shared-memory addresses stay below 256 KB, so the 14-bit field never carries).
-    const uint32_t idesc = umma_idesc_f16(kTileM, static_cast<uint32_t>(p.n_tile));
+  } else if (warp >= 4) {
+    // ================= MMA warpgroup: wgmma over the stage ring, one stage in flight behind the current one =================
+    const int tw = threadIdx.x - 128;  // thread index inside the warpgroup
+    float acc[2][NT / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) acc[h][i] = 0.f;
+    // descriptors of stage s = descriptors of stage 0 + s * (kStageBytes >> 4) in the start-address field (shared-memory
+    // addresses stay below 256 KB, so the 14-bit field never carries)
     const uint32_t sa0 = smem_u32(smem);
-    const uint64_t da0 = umma_desc_kmajor(sa0, BK * 2);
-    const uint64_t db0 = umma_desc_kmajor(sa0 + kABytes, BK * 2);
-    const uint32_t dstep = stage_bytes >> 4;
+    const uint64_t da0 = wgmma_desc_kmajor(sa0, BK * 2);
+    const uint64_t db0 = wgmma_desc_kmajor(sa0 + kABytes, BK * 2);
+    constexpr uint32_t kHalf = (64 * BK * 2) >> 4;  // pixel rows 64..127 of the A tile
+    if constexpr (STRIP) {
+      const uint64_t dw0 = wgmma_desc_kmajor(sa0, 128);                       // window 0, tap (0,0)
+      const uint64_t dbr = wgmma_desc_kmajor(sa0 + 2 * kWinStride, 128);      // weight ring, stage 0
+      RingPos rp, rw;
+      int prev = -1, prev_w = -1;
+      for (int kc = 0; kc < p.k_chunks; ++kc) {
+        mbar_wait_inline(&win_full[rw.s], rw.phase);
+        const uint64_t dwin = dw0 + static_cast<uint64_t>(rw.s * (kWinStride >> 4));
+        for (int tap = 0; tap < 9; ++tap) {
+          const int r = tap / 3, sx = tap - 3 * r;
+          mbar_wait_inline(&full_bar[rp.s], rp.phase);
+          wgmma_fence();
+          const uint64_t da = dwin + static_cast<uint64_t>((r * (kTileM + 2) + sx) * 8);   // (r rows, sx pixels) x 128 B >> 4
+          const uint64_t db = dbr + static_cast<uint64_t>(rp.s * (kStageBytes >> 4));
+#pragma unroll
+          for (int k = 0; k < BK / 16; ++k) {
+            wgmma_f16<NT, 0>(acc[0], da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k));
+            wgmma_f16<NT, 0>(acc[1], da + kHalf + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k));
+          }
+          wgmma_commit();
+          wgmma_wait<1>();  // the previous group has read its operands
+          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+          if (tap == 0 && prev_w >= 0 && lane == 0) mbar_arrive(&win_empty[prev_w]);  // last group of the previous chunk retired
+          prev = rp.s;
+          rp.advance(p.stages);
+        }
+        prev_w = rw.s;
+        rw.advance(2);
+      }
+    } else {
     RingPos rp;
     uint32_t doff = 0;
+    int prev = -1;
     for (int it = 0; it < k_iters; ++it) {
-      mbar_wait(&full_bar[rp.s], rp.phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t da = da0 + doff, db = db0 + doff;
-        // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
-        umma_f16_ss(tmem_base, da, db, idesc, it > 0 ? 1u : 0u);
+      mbar_wait_inline(&full_bar[rp.s], rp.phase);
+      wgmma_fence();
 #pragma unroll
-        for (int k = 1; k < BK / 16; ++k) umma_f16_ss(tmem_base, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), idesc, 1u);
-        umma_commit(&empty_bar[rp.s]);  // smem slot reusable once these MMAs retire
-        if (it == k_iters - 1) umma_commit(&tmem_full_bar);   // accumulator complete
+      for (int k = 0; k < BK / 16; ++k) {
+        // advance 16 fp16 = 32 B along K inside the swizzle atom: +2 in the (addr >> 4) field
+        const uint64_t da = da0 + doff + static_cast<uint64_t>(2 * k), db = db0 + doff + static_cast<uint64_t>(2 * k);
+        wgmma_f16<NT, 0>(acc[0], da, db);
+        wgmma_f16<NT, 0>(acc[1], da + kHalf, db);
       }
-      __syncwarp();
-      doff += dstep;
+      wgmma_commit();
+      wgmma_wait<1>();  // the MMAs of the previous stage have read their operands: hand that slot back to the producer
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = rp.s;
+      doff += kStageBytes >> 4;
       rp.advance(p.stages);
       if (rp.s == 0) doff = 0;
     }
-    if (p.ksplit > 1) cluster_sync_all_threads();
-  } else {
-    // ================= epilogue warps 2..5 =================
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
+    }
+    wgmma_wait<0>();
+    // park the accumulator as [channel][pixel] behind the epilogue's output area (the stage ring is idle now: every load
+    // has been consumed and every MMA has retired in all four warps once the barrier below is passed)
+    float* s_acc = reinterpret_cast<float*>(smem + conv_tc_out_bytes<NT>());
+    named_bar_sync(1, 128);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) s_acc[wgmma_col(tw, i) * kAccLd + 64 * h + wgmma_row(tw, i)] = acc[h][i];
+    named_bar_sync(1, 128);
+
+    // ================= epilogue: thread m of the warpgroup owns pixel m of the tile =================
+    const int q = warp & 3;
     const int m = q * 32 + lane;
     const int oh = h0 + m / p.tw;
     const int ow = w0 + m % p.tw;
@@ -188,51 +256,17 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
     const bool vec_ok = out_f32 ? ((reinterpret_cast<uintptr_t>(yrow32) & 15) == 0) : ((reinterpret_cast<uintptr_t>(yrow) & 15) == 0);
     const bool relu = (p.flags & FSB_CONV_RELU) != 0;
     const bool do_stats = (p.flags & FSB_CONV_STATS) != 0 && p.stats != nullptr;
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const float* part = reinterpret_cast<const float*>(smem + p.part_off);   // [ksplit - 1][n_tile][128] in CTA 0
-    if (p.ksplit > 1) {
-      if (kz > 0) {
-        // hand this CTA's partial accumulator to CTA 0: column-major [channel][pixel] so that a warp writes 128 contiguous bytes
-        const uint32_t remote = mapa_cluster(smem_u32(smem + p.part_off), 0) + static_cast<uint32_t>(kz - 1) * p.n_tile * 512u + m * 4u;
-        for (int c = 0; c < p.n_tile; c += 16) {
-          uint32_t v[16];
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) st_cluster_u32(remote + static_cast<uint32_t>(c + j) * 512u, v[j]);
-        }
-        tc_fence_before();
-      }
-      cluster_sync_all_threads();   // release / acquire: the partial sums are visible in CTA 0
-    }
-    if (kz == 0) {
-    // per-warp channel statistics of this tile: [4 warps][sum | sumsq][n_tile] in the (now idle) pipeline buffers
+    // per-warp channel statistics of this tile: [4 warps][sum | sumsq][NT] in the output area
     float* s_stat = reinterpret_cast<float*>(smem);
-    // TMEM loads are latency-bound (~250 ns per dependent tcgen05.ld + wait): issue up to four 16-column loads, wait once
-    for (int c0 = 0; c0 < p.n_tile; c0 += 64) {
-      uint32_t vv[4][16];
-      const int nb = min(4, (p.n_tile - c0) >> 4);
-#pragma unroll
-      for (int b = 0; b < 4; ++b)
-        if (b < nb) tmem_ld16(taddr + c0 + 16 * b, vv[b]);
-      tmem_ld_wait();
+    for (int c0 = 0; c0 < NT; c0 += 64) {
+      const int nb = min(4, (NT - c0) >> 4);
 #pragma unroll
       for (int b = 0; b < 4; ++b) {
       if (b >= nb) break;
       const int c = c0 + 16 * b;
-      uint32_t (&v)[16] = vv[b];
       float f[16];
 #pragma unroll
-      for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[j]);
-      if (p.ksplit > 1) {
-        for (int z = 0; z < p.ksplit - 1; ++z) {
-          const float* pz = part + (static_cast<size_t>(z) * p.n_tile + c) * 128 + m;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) f[j] += pz[j * 128];
-        }
-      }
+      for (int j = 0; j < 16; ++j) f[j] = s_acc[(c + j) * kAccLd + m];
       if (do_stats) {
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
@@ -244,8 +278,8 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
             b += __shfl_xor_sync(0xffffffffu, b, o);
           }
           if (lane == 0) {
-            s_stat[(q * 2 + 0) * p.n_tile + c + j] = a;
-            s_stat[(q * 2 + 1) * p.n_tile + c + j] = b;
+            s_stat[(q * 2 + 0) * NT + c + j] = a;
+            s_stat[(q * 2 + 1) * NT + c + j] = b;
           }
         }
       }
@@ -281,7 +315,7 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
         o1.w = pack_half2(f[14], f[15]);
         uint8_t* slab = smem + static_cast<size_t>(c0 >> 6) * (kTileM * 128);
         const int ch16 = (c - c0) >> 3;  // 16-byte chunk index inside the slab row
-        if (p.n_tile - c0 >= 64) {
+        if (NT - c0 >= 64) {
           *reinterpret_cast<uint4*>(slab + m * 128 + ((ch16 ^ (m & 7)) << 4)) = o0;
           *reinterpret_cast<uint4*>(slab + m * 128 + (((ch16 + 1) ^ (m & 7)) << 4)) = o1;
         } else {
@@ -314,250 +348,33 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
       if (p.tma_store) {
         fence_proxy_async_smem();           // generic-proxy smem writes -> visible to the TMA engine
         named_bar_sync(1, 128);             // the 4 epilogue warps
-        if (warp == 2 && lane == 0) {
-          const bool full = (p.n_tile - c0) >= 64;
+        if (warp == 4 && lane == 0) {
+          const bool full = (NT - c0) >= 64;
           tma_store_4d(&p.tmap_y[full ? 0 : 1], smem + static_cast<size_t>(c0 >> 6) * (kTileM * 128), n0 + c0, w0, h0, img);
           tma_store_commit();
         }
       }
     }  // 64-column batch
-    if (p.tma_store && warp == 2 && lane == 0) tma_store_wait_read();  // smem must outlive the bulk reads
+    if (p.tma_store && warp == 4 && lane == 0) tma_store_wait_read();  // smem must outlive the bulk reads
     if (do_stats) {
       // no atomics: the four warp partials are added in warp order and written as this tile's partial row; the consumer
       // (bn_finalize / rowsum) adds the rows in index order, so the statistics are bit-reproducible run to run
       named_bar_sync(2, 128);
       float* row = p.stats + static_cast<size_t>(blockIdx.x) * 2 * p.stats_C + p.stats_off;
-      for (int ch = static_cast<int>(threadIdx.x) - 64; ch < p.n_tile; ch += 128) {
+      for (int ch = static_cast<int>(threadIdx.x) - 128; ch < NT; ch += 128) {
         if (n0 + ch >= p.Cout) continue;
-        float a = s_stat[0 * p.n_tile + ch], b = s_stat[1 * p.n_tile + ch];
+        float a = s_stat[0 * NT + ch], b = s_stat[1 * NT + ch];
 #pragma unroll
         for (int w = 1; w < 4; ++w) {
-          a += s_stat[(w * 2 + 0) * p.n_tile + ch];
-          b += s_stat[(w * 2 + 1) * p.n_tile + ch];
+          a += s_stat[(w * 2 + 0) * NT + ch];
+          b += s_stat[(w * 2 + 1) * NT + ch];
         }
         row[n0 + ch] = a;
         row[p.stats_C + n0 + ch] = b;
       }
     }
-    }  // kz == 0
-    tc_fence_before();
   }
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// K1p: persistent variant (EXPERIMENTAL, enabled with FSB_CONV_PERSIST=1; inference epilogue only).
-//
-// The per-tile kernel above pays its prologue (barrier init, TMEM allocation, descriptor prefetch, first TMA round trip) and
-// its epilogue (TMEM -> registers -> smem -> TMA store) once per 128-pixel tile, serially with a main loop that lasts only
-// 72 MMAs for the student's largest layers -- the tensor pipe idles most of a tile's life.  Here one CTA per SM walks
-// tiles tile = blockIdx.x, += gridDim.x with
-//   * the TMA producer running ahead across tile boundaries (one continuous stage ring),
-//   * TWO accumulators in TMEM: the MMA issuer fills buffer (t & 1) while the epilogue warps drain buffer ((t - 1) & 1),
-//   * a dedicated staging buffer for the TMA store, released by cp.async.bulk.wait_group.read before it is rewritten.
-// Barriers: full/empty per stage (as above), tmem_full[2] (MMA -> epilogue, tcgen05.commit), tmem_empty[2] (epilogue ->
-// MMA, one arrival per epilogue warp after its last tcgen05.ld of the tile).
-// ------------------------------------------------------------------------------------------
-constexpr int kPersistMaxCout = 512;
-
-template <int BK>
-__global__ void __launch_bounds__(kThreads, 1)
-conv_tc_persistent_kernel(const __grid_constant__ ConvTcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t full_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
-  __shared__ __align__(8) uint64_t tmem_full_bar[2];
-  __shared__ __align__(8) uint64_t tmem_empty_bar[2];
-  __shared__ uint32_t tmem_base_smem;
-  __shared__ float s_scale[kPersistMaxCout];
-  __shared__ float s_shift[kPersistMaxCout];
-
-  pdl_launch_dependents();
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  constexpr uint32_t kABytes = kTileM * BK * 2;
-  const uint32_t b_bytes = static_cast<uint32_t>(p.n_tile) * BK * 2;
-  const uint32_t stage_bytes = kABytes + b_bytes;
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + static_cast<size_t>(p.stages) * stage_bytes;  // stage_bytes is a multiple of 1024
-  const int total_tiles = p.m_tiles * p.n_tiles;
-  const int k_iters = p.taps * p.k_chunks;
-  const uint32_t acc_cols = p.tmem_cols >> 1;  // columns of ONE accumulator (the allocation holds two)
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmap_a[0]);
-    tma_prefetch_desc(&p.tmap_b);
-    tma_prefetch_desc(&p.tmap_y[0]);
-    for (int s = 0; s < p.stages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full_bar[b], 1);
-      mbar_init(&tmem_empty_bar[b], 4);  // one arrival per epilogue warp
-    }
-    mbar_fence_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_smem, p.tmem_cols);
-    tmem_relinquish();
-  }
-  pdl_wait();
-  for (int c = threadIdx.x; c < kPersistMaxCout; c += kThreads) {
-    const bool ok = c < p.Cout;
-    s_scale[c] = (ok && (p.flags & FSB_CONV_AFFINE) && p.scale) ? p.scale[c] : 1.0f;
-    s_shift[c] = (ok && (p.flags & FSB_CONV_AFFINE) && p.shift) ? p.shift[c] : 0.0f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
-
-  if (warp == 0) {
-    // ================= TMA producer: one ring across all tiles of this CTA (converged warp, elected issue) =================
-    int it = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int n0 = (tile % p.n_tiles) * p.n_tile;
-      int t = tile / p.n_tiles;
-      const int w0 = (t % p.tiles_w) * p.tw;
-      t /= p.tiles_w;
-      const int h0 = (t % p.tiles_h) * p.th;
-      const int img = t / p.tiles_h;
-      for (int tap = 0; tap < p.taps; ++tap) {
-        const CUtensorMap* ma = &p.tmap_a[p.tap_map[tap]];
-        const int cw = w0 + p.tap_dw[tap];
-        const int chh = h0 + p.tap_dh[tap];
-        for (int kc = 0; kc < p.k_chunks; ++kc, ++it) {
-          const int s = it % p.stages;
-          const int round = it / p.stages;
-          if (round > 0) mbar_wait(&empty_bar[s], (round - 1) & 1);
-          uint8_t* sa = smem + static_cast<size_t>(s) * stage_bytes;
-          uint8_t* sb = sa + kABytes;
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&full_bar[s], stage_bytes);
-            tma_load_4d(sa, ma, &full_bar[s], kc * BK, cw, chh, img);
-            tma_load_3d(sb, &p.tmap_b, &full_bar[s], kc * BK, n0, p.tap_widx[tap]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================= MMA issuer: alternates between the two TMEM accumulators =================
-    const uint32_t idesc = umma_idesc_f16(kTileM, static_cast<uint32_t>(p.n_tile));
-    int it = 0;
-    int lt = 0;  // tiles done by this CTA
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-      const int buf = lt & 1;
-      const int use = lt >> 1;  // how often this accumulator has been used before
-      if (use > 0) mbar_wait(&tmem_empty_bar[buf], (use - 1) & 1);  // epilogue of its previous tile has drained it
-      tc_fence_after();
-      const uint32_t acc = tmem_base + static_cast<uint32_t>(buf) * acc_cols;
-      for (int ki = 0; ki < k_iters; ++ki, ++it) {
-        const int s = it % p.stages;
-        const int round = it / p.stages;
-        mbar_wait(&full_bar[s], round & 1);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + static_cast<size_t>(s) * stage_bytes);
-        const uint32_t sb = sa + kABytes;
-        const uint64_t da = umma_desc_kmajor(sa, BK * 2);
-        const uint64_t db = umma_desc_kmajor(sb, BK * 2);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_f16_ss(acc, da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k), idesc, (ki > 0 || k > 0) ? 1u : 0u);
-          umma_commit(&empty_bar[s]);
-          if (ki == k_iters - 1) umma_commit(&tmem_full_bar[buf]);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ================= epilogue warps 2..5: drain accumulator (t & 1) while the MMA warp fills the other =================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;
-    const bool relu = (p.flags & FSB_CONV_RELU) != 0;
-    int lt = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-      const int buf = lt & 1;
-      const int use = lt >> 1;
-      const int n0 = (tile % p.n_tiles) * p.n_tile;
-      int t = tile / p.n_tiles;
-      const int w0 = (t % p.tiles_w) * p.tw;
-      t /= p.tiles_w;
-      const int h0 = (t % p.tiles_h) * p.th;
-      const int img = t / p.tiles_h;
-      mbar_wait(&tmem_full_bar[buf], use & 1);
-      tc_fence_after();
-      if (lt > 0) {
-        // the staging buffer still feeds the previous tile's bulk stores until they have READ it
-        if (warp == 2 && lane == 0) tma_store_wait_read();
-        named_bar_sync(1, 128);
-      }
-      const uint32_t taddr = tmem_base + static_cast<uint32_t>(buf) * acc_cols + (static_cast<uint32_t>(q * 32) << 16);
-      for (int c0 = 0; c0 < p.n_tile; c0 += 64) {
-        uint32_t vv[4][16];
-        const int nb = min(4, (p.n_tile - c0) >> 4);
-#pragma unroll
-        for (int b = 0; b < 4; ++b)
-          if (b < nb) tmem_ld16(taddr + c0 + 16 * b, vv[b]);
-        tmem_ld_wait();
-        if (c0 + 64 >= p.n_tile) {
-          // last TMEM read of this tile by this warp: hand the accumulator back to the MMA issuer
-          tc_fence_before();
-          if (lane == 0) mbar_arrive(&tmem_empty_bar[buf]);
-        }
-        uint8_t* slab = staging + static_cast<size_t>(c0 >> 6) * (kTileM * 128);
-        const bool full_slab = (p.n_tile - c0) >= 64;
-#pragma unroll
-        for (int b = 0; b < 4; ++b) {
-          if (b >= nb) break;
-          const int c = c0 + 16 * b;
-          float f[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float x = __uint_as_float(vv[b][j]) * s_scale[n0 + c + j] + s_shift[n0 + c + j];
-            f[j] = relu ? fmaxf(x, 0.f) : x;
-          }
-          uint4 o0, o1;
-          o0.x = pack_half2(f[0], f[1]);
-          o0.y = pack_half2(f[2], f[3]);
-          o0.z = pack_half2(f[4], f[5]);
-          o0.w = pack_half2(f[6], f[7]);
-          o1.x = pack_half2(f[8], f[9]);
-          o1.y = pack_half2(f[10], f[11]);
-          o1.z = pack_half2(f[12], f[13]);
-          o1.w = pack_half2(f[14], f[15]);
-          const int ch16 = (c - c0) >> 3;
-          if (full_slab) {
-            *reinterpret_cast<uint4*>(slab + m * 128 + ((ch16 ^ (m & 7)) << 4)) = o0;
-            *reinterpret_cast<uint4*>(slab + m * 128 + (((ch16 + 1) ^ (m & 7)) << 4)) = o1;
-          } else {
-            uint8_t* row = slab + m * (p.tail_w * 2) + (ch16 << 4);
-            *reinterpret_cast<uint4*>(row) = o0;
-            *reinterpret_cast<uint4*>(row + 16) = o1;
-          }
-        }
-        fence_proxy_async_smem();
-        named_bar_sync(1, 128);
-        if (warp == 2 && lane == 0) {
-          tma_store_4d(&p.tmap_y[full_slab ? 0 : 1], slab, n0 + c0, w0, h0, img);
-          tma_store_commit();
-        }
-      }
-    }
-    if (warp == 2 && lane == 0) tma_store_wait_read();
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -610,8 +427,18 @@ ConvGeom conv_geom(const fsb_conv_desc* d) {
   return g;
 }
 
-// spatial tiles (= CTAs along M = partial statistic rows) of the per-tap kernel
+// Row-strip mode (see conv_tc_kernel): 3x3 stride-1 dilation-1 inference convs with 64-channel chunks, only with
+// FSB_CONV_TC2=2.  Off by default: on H100 it is slower than the per-tap mode on every 3x3 layer of the student frame (1.07-2x,
+// heads8 even) -- one CTA per SM (two 50 KB input windows) cannot hide its epilogue behind a second CTA, and the per-tap
+// mode's 9x input re-reads are served by L2 (tools/conv_bench.py --compare-strip, DESIGN.md section 3.3).
+bool conv_tc_strip(const fsb_conv_desc* d) {
+  if (d->ksize != 3 || d->stride != 1 || d->dil != 1 || d->Cin % 64 != 0 || (d->flags & FSB_CONV_STATS)) return false;
+  return opt(OPT_CONV_TC2) == 2;
+}
+
+// spatial tiles (= CTAs along M = partial statistic rows) of conv_tc
 int conv_tc_m_tiles(const fsb_conv_desc* d) {
+  if (conv_tc_strip(d)) return ((d->Wo + kTileM - 1) / kTileM) * d->Ho * d->N;
   const int tw = d->Wo >= 16 ? 16 : 8, th = kTileM / tw;
   return ((d->Wo + tw - 1) / tw) * ((d->Ho + th - 1) / th) * d->N;
 }
@@ -620,6 +447,26 @@ int conv_tc_supported(const fsb_conv_desc* d) {
   if (d->Cin < 16 || (d->x_cstride % 8) != 0) return 0;
   if (!(d->ksize == 1 || d->ksize == 3) || !(d->stride == 1 || d->stride == 2)) return 0;
   return 1;
+}
+
+template <int BK, int NT, bool STRIP = false>
+static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcParams& p) {
+  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, STRIP>), 220 * 1024, "cudaFuncSetAttribute(conv_tc)"))
+    return rc;
+  const cudaError_t e = launch_kernel(conv_tc_kernel<BK, NT, STRIP>, grid, dim3(kThreads), smem_bytes, stream, p);
+  return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
+}
+
+template <int BK, bool STRIP>
+static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcParams& p) {
+  switch (n_tile) {
+    case 16: return conv_tc_run<BK, 16, STRIP>(grid, smem_bytes, stream, p);
+    case 32: return conv_tc_run<BK, 32, STRIP>(grid, smem_bytes, stream, p);
+    case 48: return conv_tc_run<BK, 48, STRIP>(grid, smem_bytes, stream, p);
+    case 64: return conv_tc_run<BK, 64, STRIP>(grid, smem_bytes, stream, p);
+    case 96: return conv_tc_run<BK, 96, STRIP>(grid, smem_bytes, stream, p);
+    default: return conv_tc_run<BK, 128, STRIP>(grid, smem_bytes, stream, p);
+  }
 }
 
 int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
@@ -635,27 +482,32 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   p.k_chunks = g.kpad / g.bk;
   p.Ho = cu ? cu->Ho : d->Ho;
   p.Wo = cu ? cu->Wo : d->Wo;
-  p.tw = p.Wo >= 16 ? 16 : 8;
+  const bool strip = !cu && conv_tc_strip(d);
+  p.tw = strip ? kTileM : (p.Wo >= 16 ? 16 : 8);
   p.th = kTileM / p.tw;
   p.tiles_w = (p.Wo + p.tw - 1) / p.tw;
   p.tiles_h = (p.Ho + p.th - 1) / p.th;
   for (int i = 0; i < 9; ++i) p.tap_widx[i] = i;
   p.Cout = d->Cout;
-  // Output-channel tiling.  Default: one N tile (<= 256 columns).  When the spatial tiling alone cannot fill the
-  // machine (small maps at 1/16, 1/32 resolution), split N further so that more SMs pull operands from L2 in parallel
-  // (each CTA then streams A 16 KB + a thinner B slab per k-step).  B boxes past npad rows are zero-filled by TMA.
+  // Output-channel tiling: N tiles of 16, 32, 48, 64, 96 or 128 channels (the wgmma N of the kernel instance; B boxes past npad
+  // rows are zero-filled by TMA and the epilogue stores only channels < Cout): the fewest tiles of <= 128, each the smallest
+  // instance that covers its share.  When the spatial tiling alone cannot fill the machine (small maps at 1/16, 1/32
+  // resolution), split N further so that more SMs pull operands from L2 in parallel.
+  static const int kNt[] = {16, 32, 48, 64, 96, 128};
   const int m_tiles = p.tiles_w * p.tiles_h * d->N;
-  int n_tiles = (g.npad + 255) / 256;
-  int n_tile = ((g.npad + n_tiles - 1) / n_tiles + 15) / 16 * 16;
+  int n_tiles = (g.npad + 127) / 128;
+  int ni = 0;
+  while (kNt[ni] * n_tiles < g.npad) ++ni;
+  int n_tile = kNt[ni];
+  n_tiles = (g.npad + n_tile - 1) / n_tile;
   const int sms = sm_count();
-  // FSB_CONV_NTILE_MIN: smallest N tile the split may produce (default 32).  An MMA costs about the same whatever its N (DESIGN 3.1),
-  // so splitting N does not shorten a CTA's main loop; it only spreads the weight loads and the epilogue over more SMs.
+  // FSB_CONV_NTILE_MIN: smallest N tile the split may produce (default 32).  Splitting N does not shorten a CTA's main loop
+  // (every tap and channel chunk is still walked); it spreads the weight loads and the epilogue over more SMs.
   const int nt_min = opt(OPT_CONV_NTILE_MIN) >= 16 ? opt(OPT_CONV_NTILE_MIN) : 32;
-  while (m_tiles * n_tiles < sms && n_tile > nt_min) {
-    n_tile = (n_tile / 2 + 15) / 16 * 16;
+  while (m_tiles * n_tiles < sms && ni > 0 && kNt[ni - 1] >= nt_min) {
+    n_tile = kNt[--ni];
     n_tiles = (g.npad + n_tile - 1) / n_tile;
   }
-  p.n_tile = n_tile;
   p.y_cstride = d->y_cstride;
   p.flags = d->flags;
   p.scale = scale;
@@ -666,40 +518,22 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   p.stats_off = d->stats_off;
   if ((d->flags & FSB_CONV_STATS) && stats && (d->stats_off < 0 || d->stats_off + d->Cout > p.stats_C))
     return set_error(FSB_ERR_INVALID, "conv_tc: stats_off + Cout exceeds stats_C");
-  uint32_t cols = 32;
-  while (cols < static_cast<uint32_t>(n_tile)) cols <<= 1;
-  p.tmem_cols = cols;
 
-  const size_t stage_bytes = static_cast<size_t>(kTileM) * g.bk * 2 + static_cast<size_t>(n_tile) * g.bk * 2;
+  const size_t stage_bytes = (strip ? 0 : static_cast<size_t>(kTileM) * g.bk * 2) + static_cast<size_t>(n_tile) * g.bk * 2;
   const int k_iters = p.taps * p.k_chunks;
-  // <= one CTA per SM anyway -> give the pipeline (almost) the whole shared memory; otherwise keep 2 CTAs/SM resident
-  const size_t smem_budget = (m_tiles * n_tiles <= sms) ? 192 * 1024 : 96 * 1024;
-  int stages = static_cast<int>(smem_budget / stage_bytes);
+  // 128-channel tiles hold 128 accumulator registers per thread: one CTA per SM, give the pipeline (almost) the whole shared
+  // memory; the same when the grid has at most one CTA per SM anyway.  Otherwise keep two CTAs per SM resident.
+  const size_t smem_budget = (n_tile == 128 || m_tiles * n_tiles <= sms) ? 200 * 1024 : 100 * 1024;
+  const size_t win_bytes = strip ? 2 * kWinStride : 0;   // row strip: two input windows ahead of the weight ring
+  int stages = static_cast<int>((strip ? 200 * 1024 - win_bytes : smem_budget) / stage_bytes);
   if (stages < 2) stages = 2;
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages > k_iters) stages = k_iters;
-  // ---- split-K over a 3-CTA cluster (one kernel row per CTA) for small maps: the serial MMA chain of a tile shrinks 3x ----
-  p.ksplit = 1;
-  // Default OFF (FSB_CONV_KSPLIT=1 turns it on): measured on B200 it shortens an isolated small conv by 15-30 % (cell9-0.conv2
-  // 10.3 -> 7.1 us) but inside the frame and the supernet step the small convs of independent branches already overlap on side
-  // streams, and tripling their CTA count costs more concurrency than the shorter chains win (frame 0.393 -> 0.411 ms, pretrain step
-  // 170 -> 191 ms; profiles/r2_conv_bench_ksplit.log).
-  if (!cu && g.taps == 9 && opt(OPT_CONV_KSPLIT) > 0 && m_tiles * n_tiles * 3 <= sms && n_tile <= 128) {
-    const size_t part_bytes = static_cast<size_t>(2) * n_tile * 512;
-    const size_t room = 216 * 1024 - part_bytes;
-    int st3 = static_cast<int>(room / stage_bytes);
-    const int k_local = 3 * p.k_chunks;
-    if (st3 > kMaxStages) st3 = kMaxStages;
-    if (st3 > k_local) st3 = k_local;
-    if (st3 >= 2 || (st3 >= 1 && k_local == 1)) {
-      p.ksplit = 3;
-      stages = st3;
-      p.part_off = static_cast<uint32_t>(stage_bytes * stages);
-    }
-  }
   p.stages = stages;
-  size_t smem_bytes = stage_bytes * stages + 1024;
-  if (p.ksplit > 1) smem_bytes += static_cast<size_t>(2) * n_tile * 512;
+  const size_t epi_bytes = n_tile == 16 ? conv_tc_epilogue_bytes<16>() : n_tile == 32 ? conv_tc_epilogue_bytes<32>()
+                           : n_tile == 48 ? conv_tc_epilogue_bytes<48>() : n_tile == 64 ? conv_tc_epilogue_bytes<64>()
+                           : n_tile == 96 ? conv_tc_epilogue_bytes<96>() : conv_tc_epilogue_bytes<128>();
+  size_t smem_bytes = (win_bytes + stage_bytes * stages > epi_bytes ? win_bytes + stage_bytes * stages : epi_bytes) + 1024;
   // ---- TMA-store epilogue: fp16 output whose pixels start on 16 B and whose channel count is a multiple of 8 ----
   p.tma_store = 0;
   if (!(d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS)) && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
@@ -724,15 +558,14 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     if (rc) return rc;
     if (n_tile < 64) p.tmap_y[0] = p.tmap_y[1];
     p.tma_store = 1;
-    const size_t staging = static_cast<size_t>((n_tile + 63) / 64) * kTileM * 128 + 1024;
-    if (smem_bytes < staging) smem_bytes = staging;
   }
   if (cu && !p.tma_store) return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: custom output lattice needs the TMA-store epilogue");
 
   // ---- A tensor maps ----
   const __half* xb = static_cast<const __half*>(x);
   const uint64_t cs = static_cast<uint64_t>(d->x_cstride) * 2;  // bytes per pixel step
-  const uint32_t boxA[4] = {static_cast<uint32_t>(g.bk), static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
+  const uint32_t boxA[4] = {static_cast<uint32_t>(g.bk), static_cast<uint32_t>(strip ? kTileM + 2 : p.tw),
+                            static_cast<uint32_t>(strip ? 3 : p.th), 1u};
   if (d->stride == 1) {
     const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
                               static_cast<uint64_t>(d->N)};
@@ -789,66 +622,10 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     int rc = encode_tiled(&p.tmap_b, wpacked, 3, dims, str, boxB, g.bk * 2);
     if (rc) return rc;
   }
-  cudaError_t e;
-  // ---- experimental persistent variant (see K1p above): inference epilogue, plain taps, several tiles per SM ----
-  const bool persist_on = opt(OPT_CONV_PERSIST) == 1;
-  if (persist_on && !cu && p.tma_store && d->Cout <= kPersistMaxCout && !(d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS)) &&
-      m_tiles * n_tiles > sms && cols <= 256) {
-    const size_t staging = static_cast<size_t>((n_tile + 63) / 64) * kTileM * 128;
-    // tuning knobs for the first measurements: CTAs per SM (1 = whole shared memory for one pipeline, 2 = two issuers
-    // sharing the tensor core, TMEM 2 x 2 x cols <= 512) and a cap on the pipeline depth
-    const int occ_env = opt(OPT_PERSIST_OCC) == 2 ? 2 : 1;
-    const int stages_env = opt(OPT_PERSIST_STAGES) > 0 ? opt(OPT_PERSIST_STAGES) : 0;
-    const int occ = (occ_env == 2 && cols * 4 <= 512) ? 2 : 1;
-    const size_t budget = (occ == 2 ? 100 : 200) * 1024;
-    int pst = budget > staging ? static_cast<int>((budget - staging) / stage_bytes) : 0;
-    if (pst > kMaxStages) pst = kMaxStages;
-    if (stages_env >= 2 && pst > stages_env) pst = stages_env;
-    if (pst >= 2) {
-      p.m_tiles = m_tiles;
-      p.n_tiles = n_tiles;
-      p.tmem_cols = cols * 2;  // two accumulators
-      p.stages = pst;
-      const size_t psmem = stage_bytes * pst + staging + 1024;
-      const unsigned ctas = static_cast<unsigned>(m_tiles * n_tiles < sms * occ ? m_tiles * n_tiles : sms * occ);
-      if (g.bk == 64) {
-        if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_persistent_kernel<64>), 216 * 1024, "cudaFuncSetAttribute(conv_tc_persistent<64>)")) return rc;
-        e = launch_kernel(conv_tc_persistent_kernel<64>, dim3(ctas), dim3(kThreads), psmem, stream, p);
-      } else {
-        if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_persistent_kernel<32>), 216 * 1024, "cudaFuncSetAttribute(conv_tc_persistent<32>)")) return rc;
-        e = launch_kernel(conv_tc_persistent_kernel<32>, dim3(ctas), dim3(kThreads), psmem, stream, p);
-      }
-      if (e != cudaSuccess) return set_cuda_error(e, "conv_tc persistent launch");
-      return FSB_OK;
-    }
-  }
-  dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles), static_cast<unsigned>(p.ksplit));
-  if (int rc = ensure_dyn_smem(g.bk == 64 ? reinterpret_cast<const void*>(conv_tc_kernel<64>) : reinterpret_cast<const void*>(conv_tc_kernel<32>),
-                               220 * 1024, "cudaFuncSetAttribute(conv_tc)")) return rc;
-  if (p.ksplit > 1) {
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = static_cast<unsigned>(p.ksplit);
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    e = g.bk == 64 ? cudaLaunchKernelEx(&cfg, conv_tc_kernel<64>, p) : cudaLaunchKernelEx(&cfg, conv_tc_kernel<32>, p);
-  } else if (g.bk == 64) {
-    e = launch_kernel(conv_tc_kernel<64>, grid, dim3(kThreads), smem_bytes, stream, p);
-  } else {
-    e = launch_kernel(conv_tc_kernel<32>, grid, dim3(kThreads), smem_bytes, stream, p);
-  }
-  if (e != cudaSuccess) return set_cuda_error(e, "conv_tc launch");
-  return FSB_OK;
+  const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles));
+  if (strip) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, p);
+  if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, p);
+  return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, p);
 }
 
 }  // namespace fsb

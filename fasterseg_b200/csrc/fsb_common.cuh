@@ -1,7 +1,6 @@
-// fsb_common.cuh -- sm_100a PTX wrappers (mbarrier, TMA, tcgen05/TMEM) shared by the kernels.
-// Hand-written for B200; no CUTLASS dependency.  Bit layouts of the UMMA shared-memory and
-// instruction descriptors follow the PTX ISA (tcgen05 "matrix descriptor" / "instruction
-// descriptor" tables).
+// fsb_common.cuh -- sm_90a PTX wrappers (mbarrier, TMA, clusters, wgmma) shared by the kernels.
+// Hand-written for H100; no CUTLASS dependency.  The bit layout of the wgmma shared-memory matrix
+// descriptor follows the PTX ISA ("Matrix Descriptor Format" of the asynchronous warpgroup MMA).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -60,9 +59,8 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must surface as a launch failure, never as a hung GPU.  The slow path lives out of line: the
-// waits sit inside the single-warp TMA / MMA issue loops, whose instruction count per iteration bounds the tensor-pipe feed
-// rate (tools/umma_rate.cu: ~50 dependent instructions cost as much as two 128x128x16 MMAs).
+// Bounded wait: a protocol bug must surface as a launch failure, never as a hung GPU.  The slow path lives out of line so
+// that the waits inside the TMA producer and MMA loops stay short.
 static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity) {
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
@@ -75,6 +73,13 @@ static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parit
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   mbar_wait_slow(bar, parity);
+}
+// Same bound without the out-of-line call: for waits while wgmma groups are in flight (a call there makes ptxas serialize
+// every wgmma of the kernel).
+__device__ __forceinline__ void mbar_wait_inline(uint64_t* bar, uint32_t parity) {
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 4000000000LL) __trap();
 }
 // Position in a ring of `n` stages with the phase parity of the current round; advanced without integer division.
 // Consumer side: wait(full[s], phase).  Producer side: wait(empty[s], phase ^ 1) -- on a freshly initialised barrier the
@@ -144,82 +149,95 @@ __device__ __forceinline__ void st_cluster_u32(uint32_t cluster_addr, uint32_t v
 }
 
 // ------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, load
+// wgmma: warpgroup-collective D[64 x N] += A[64 x 16] * B[N x 16]^T, fp16 inputs from shared memory, fp32 accumulator in
+// registers.  Thread t of the warpgroup (warp w = t / 32, lane l) holds, for i in [0, N/2):
+//   row 16 * w + l / 4 + 8 * ((i >> 1) & 1),  column 8 * (i >> 2) + 2 * (l & 3) + (i & 1)
+// (wgmma_row / wgmma_col).  TR = 0: both operands K-major; TR = 1: both MN-major.  The accumulator is always added to
+// (scale-d = 1): callers zero it before the first K step.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ int wgmma_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int wgmma_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
 
-// D[tmem] (+)= A[smem] * B[smem], fp16 inputs, fp32 accumulate, issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
+template <int TR>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, %10, %11;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "n"(TR), "n"(TR));
 }
-// All previously issued MMAs of this thread arrive (once) on `bar` when they complete.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// TMEM -> registers: warp-collective; thread t of the warp reads lane (lane_base + t), 16 consecutive
-// 32-bit columns starting at the column encoded in taddr.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
+template <int TR>
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1, 1, 1, %18, %19;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "n"(TR), "n"(TR));
 }
-// same, 32 consecutive columns
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+template <int TR>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]),
-        "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]),
-        "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, %34, %35;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "n"(TR), "n"(TR));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <int TR>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 1, 1, 1, %66, %67;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "n"(TR), "n"(TR));
+}
 
-// UMMA shared-memory matrix descriptor, K-major operand, rows of `row_bytes` (32/64/128) bytes
-// written by TMA with the matching swizzle mode.
-//   bits [0,14)  start address >> 4          bits [16,30) leading byte offset >> 4 (unused for swizzled K-major)
-//   bits [32,46) stride byte offset >> 4 (distance between 8-row groups = 8 * row_bytes)
-//   bits [46,48) descriptor version = 1 (Blackwell)   bits [61,64) layout: 2 = SW128, 4 = SW64, 6 = SW32
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr, uint32_t row_bytes) {
-  const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
+template <int TR>
+__device__ __forceinline__ void wgmma_m64n48k16(float (&d)[24], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n48k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, 1, 1, 1, %26, %27;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(da), "l"(db), "n"(TR), "n"(TR));
+}
+template <int TR>
+__device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t da, uint64_t db) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, 1, 1, 1, %50, %51;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(da), "l"(db), "n"(TR), "n"(TR));
+}
+
+template <int N, int TR>
+__device__ __forceinline__ void wgmma_f16(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  if constexpr (N == 16) wgmma_m64n16k16<TR>(d, da, db);
+  else if constexpr (N == 32) wgmma_m64n32k16<TR>(d, da, db);
+  else if constexpr (N == 48) wgmma_m64n48k16<TR>(d, da, db);
+  else if constexpr (N == 64) wgmma_m64n64k16<TR>(d, da, db);
+  else if constexpr (N == 96) wgmma_m64n96k16<TR>(d, da, db);
+  else wgmma_m64n128k16<TR>(d, da, db);
+}
+
+// wgmma shared-memory matrix descriptor, swizzled layout written by TMA (or by hand in the same pattern):
+//   bits [0,14)  start address >> 4          bits [16,30) leading byte offset >> 4
+//   bits [32,46) stride byte offset >> 4     bits [62,64) layout: 1 = SW128, 2 = SW64, 3 = SW32
+// K-major operand with rows of `row_bytes` (32/64/128) bytes: the leading offset is unused, the stride offset is the distance
+// between 8-row groups (8 * row_bytes).  Advancing 16 fp16 along K inside the swizzle atom adds 2 to the address field.
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swizzle_bytes) {
+  const uint64_t layout = swizzle_bytes == 128 ? 1ull : (swizzle_bytes == 64 ? 2ull : 3ull);
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>((8u * row_bytes) >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= layout << 61;
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
+  d |= layout << 62;
   return d;
 }
-// Instruction descriptor for kind::f16: fp16 A/B (format 0), fp32 accumulate (c_format 1), both K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor(uint32_t smem_addr, uint32_t row_bytes) {
+  return wgmma_desc(smem_addr, 16, 8 * row_bytes, row_bytes);
 }
 
 // ------------------------------------------------------------------------------------------

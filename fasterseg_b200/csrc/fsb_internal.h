@@ -32,23 +32,24 @@ bool pdl_enabled();
 int sm_count();
 
 // Tuning / validation switches.  Read from the environment ONCE (first use) and settable through fsb_set_option(); never a
-// getenv() on the launch path.  -1 = unset.
+// getenv() on the launch path.  -1 = unset.  The switches marked "no effect" selected conv kernel variants that this sm_90a
+// library does not have; their names stay accepted so that existing settings keep working.
 enum Opt {
-  OPT_CONV_TC2 = 0,      // FSB_CONV_TC2: 0 = never use the row-strip kernel, 2 = force it wherever it is supported
-  OPT_TC2_R,             // FSB_TC2_R: rows per CTA override
-  OPT_TC2_ASTAGES,       // FSB_TC2_ASTAGES
+  OPT_CONV_TC2 = 0,      // FSB_CONV_TC2: 2 = row-strip mode of conv_tc wherever the geometry allows (default: per-tap)
+  OPT_TC2_R,             // FSB_TC2_R: no effect
+  OPT_TC2_ASTAGES,       // FSB_TC2_ASTAGES: no effect
   OPT_NO_TMA_STORE,      // FSB_NO_TMA_STORE
   OPT_DGRAD_S2_DIRECT,   // FSB_DGRAD_S2_DIRECT
   OPT_WGRAD_TC,          // FSB_WGRAD_TC: 0 = CUDA-core weight gradient
-  OPT_CONV_PERSIST,      // FSB_CONV_PERSIST
-  OPT_PERSIST_OCC,       // FSB_PERSIST_OCC
-  OPT_PERSIST_STAGES,    // FSB_PERSIST_STAGES
+  OPT_CONV_PERSIST,      // FSB_CONV_PERSIST: no effect
+  OPT_PERSIST_OCC,       // FSB_PERSIST_OCC: no effect
+  OPT_PERSIST_STAGES,    // FSB_PERSIST_STAGES: no effect
   OPT_UPSAMPLE_V2,       // FSB_UPSAMPLE_V2
   OPT_DETERMINISTIC,     // FSB_DETERMINISTIC: 1 = weight gradients without split-K atomics (bit-reproducible steps)
-  OPT_CONV_TC3,          // FSB_CONV_TC3: 0 = never use the channel-major 128x256 kernel, 2 = force it wherever it is supported
-  OPT_CONV_TC4,          // FSB_CONV_TC4: 0 = never use the CTA-pair row-rolling kernel, 2 = force it wherever it is supported
-  OPT_CONV_TC5,          // FSB_CONV_TC5: 0 = never use the tap-concatenated kernel (Cout <= 64), 2 = force it wherever it is supported
-  OPT_CONV_KSPLIT,       // FSB_CONV_KSPLIT: 1 = split a 3x3 tile's K over a 3-CTA cluster (conv_tc on small maps); default off
+  OPT_CONV_TC3,          // FSB_CONV_TC3: no effect
+  OPT_CONV_TC4,          // FSB_CONV_TC4: no effect
+  OPT_CONV_TC5,          // FSB_CONV_TC5: no effect
+  OPT_CONV_KSPLIT,       // FSB_CONV_KSPLIT: no effect
   OPT_CONV_NTILE_MIN,    // FSB_CONV_NTILE_MIN: lower bound of the output-channel tile when conv_tc splits N to occupy more SMs (default 32)
   OPT_COUNT
 };
@@ -98,30 +99,9 @@ struct ConvTcCustom {
   uint64_t y_strides[3];  // bytes: lattice step in W, in H, image
 };
 int conv_tc_supported(const fsb_conv_desc* d);
+bool conv_tc_strip(const fsb_conv_desc* d);  // conv_tc runs d in row-strip mode
 int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
                    void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr);
-int conv_tc2_supported(const fsb_conv_desc* d);
-int conv_tc2_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                    void* y, float* stats, cudaStream_t stream);
-int conv_tc3_supported(const fsb_conv_desc* d, const void* y);
-int conv_tc3_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift, void* y,
-                    cudaStream_t stream);
-int conv_tc5_supported(const fsb_conv_desc* d, const void* y);
-int conv_tc5_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift, void* y,
-                    cudaStream_t stream);
-int conv_tc4_supported(const fsb_conv_desc* d, const void* y);
-int conv_tc4_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift, void* y,
-                    cudaStream_t stream);
-// picks the CTA-pair row-rolling kernel for the big 3x3 stride-1 inference convs, the channel-major 128x256 kernel for wide-Cout inference / dgrad convs, the row-strip kernel for wide 3x3 stride-1
-// convs with few output channels, the per-tap kernel otherwise
-inline int conv_tc_dispatch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                            void* y, float* stats, cudaStream_t stream) {
-  if (!stats && conv_tc5_supported(d, y)) return conv_tc5_launch(d, x, wpacked, scale, shift, y, stream);
-  if (!stats && conv_tc4_supported(d, y)) return conv_tc4_launch(d, x, wpacked, scale, shift, y, stream);
-  if (!stats && conv_tc3_supported(d, y)) return conv_tc3_launch(d, x, wpacked, scale, shift, y, stream);
-  if (conv_tc2_supported(d)) return conv_tc2_launch(d, x, wpacked, scale, shift, y, stats, stream);
-  return conv_tc_launch(d, x, wpacked, scale, shift, y, stats, stream);
-}
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride);
 int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
                          float gscale, cudaStream_t stream);

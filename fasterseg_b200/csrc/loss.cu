@@ -427,7 +427,7 @@ int loss_check(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int 
   return FSB_OK;
 }
 
-constexpr int kLossRows = 1184;   // 8 x 148 partial rows
+constexpr int kLossRows = 1056;   // 8 x 132 partial rows
 
 }  // namespace
 

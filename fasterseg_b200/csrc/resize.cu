@@ -579,7 +579,7 @@ int copy_channels_launch(int64_t pixels, int C, const void* x, int xcs, void* y,
     return set_error(FSB_ERR_INVALID, "copy_channels: C, strides must be multiples of 8 and pointers 16B aligned");
   const int64_t total = pixels * (C / 8);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   FSB_LAUNCH(copy_channels_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream, pixels, C / 8, static_cast<const __half*>(x), xcs,
                                                                         static_cast<__half*>(y), ycs);
   cudaError_t e = last_launch_error();

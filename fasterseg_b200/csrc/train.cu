@@ -203,7 +203,7 @@ static inline bool vec_ok(int C, int cs, const void* p) { return C % 8 == 0 && c
 static inline unsigned grid_for(int64_t total, int threads) {
   int64_t b = (total + threads - 1) / threads;
   if (b < 1) b = 1;
-  if (b > 148 * 16) b = 148 * 16;
+  if (b > 132 * 16) b = 132 * 16;
   return static_cast<unsigned>(b);
 }
 
@@ -269,7 +269,7 @@ int relu_bwd_launch(int64_t pixels, int C, const void* dy, int dcs, const void* 
 // ------------------------------------------------------------------------------------------
 // conv dgrad
 // ------------------------------------------------------------------------------------------
-// weights for the tcgen05 path: the data gradient of a stride-1 conv is itself a stride-1 conv of dy with the
+// weights for the tensor-core path: the data gradient of a stride-1 conv is itself a stride-1 conv of dy with the
 // spatially flipped, channel-transposed filter: packed_t[tap'][n = ci][k = co] = w[co][ci][K-1-r'][K-1-s']
 __global__ void pack_dgrad_kernel(const float* __restrict__ w, int64_t so, int64_t si, int ks, int Cout, int Cin, int npad,
                                   int kpad, __half* __restrict__ out) {
@@ -378,7 +378,7 @@ int conv_dgrad_launch(const fsb_conv_desc* d, const void* dy, int dcs, const voi
                       int64_t si, void* dx, int xcs, cudaStream_t stream) {
   if (d->stride == 1 && d->off_h == 0 && d->off_w == 0 && wpacked_t && !(d->flags & FSB_CONV_FORCE_DIRECT)) {
     fsb_conv_desc t = dgrad_as_fwd_desc(d, dcs, xcs);
-    if (conv_tc_supported(&t)) return conv_tc_dispatch(&t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream);
+    if (conv_tc_supported(&t)) return conv_tc_launch(&t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream);
   }
   // stride 2: the input pixels of each (row, column) parity receive contributions from a fixed subset of filter taps; each
   // parity plane is a stride-1 implicit GEMM over dy with that tap subset, written to the plane through a strided tensor map
@@ -573,7 +573,7 @@ int conv_wgrad_launch(const fsb_conv_desc* d, const void* x, const void* dy, int
   const int64_t npix = static_cast<int64_t>(d->N) * d->Ho * d->Wo;
   const int tiles = ((d->Cout + kWgTile - 1) / kWgTile) * ((d->Cin + kWgTile - 1) / kWgTile) * taps;
   // enough pixel chunks to fill the machine a few times over, each at least 256 pixels
-  int64_t chunks = (148 * 4 + tiles - 1) / tiles;
+  int64_t chunks = (132 * 4 + tiles - 1) / tiles;
   const int64_t max_chunks = (npix + 255) / 256;
   if (chunks > max_chunks) chunks = max_chunks;
   if (chunks < 1 || opt(OPT_DETERMINISTIC) == 1) chunks = 1;  // deterministic mode: one owner per output element, no split-K atomics
@@ -821,7 +821,7 @@ wsum_bwd_kernel(const WsumArgs a, int64_t pixels, int cvec, const __half* __rest
 int wsum_rows(int64_t pixels, int C) {
   int64_t b = (pixels * (C / 8) + 255) / 256;
   if (b < 1) b = 1;
-  if (b > 148 * 2) b = 148 * 2;
+  if (b > 132 * 2) b = 132 * 2;
   return static_cast<int>(b);
 }
 int wsum_fwd_launch(int K, int64_t pixels, int C, const void* const* xs, const int* xcs, const float* wts, void* out, int ocs,

@@ -16,7 +16,6 @@ int bn_bwd_apply_launch(int64_t, int, const void*, int, const void*, int, const 
                         const fsb_bn_sel*, const int*, int, const float*);
 int rowsum_launch(int, const float*, int, int, float*, cudaStream_t);
 int conv_tc_m_tiles(const fsb_conv_desc*);
-int conv_tc2_ctas(const fsb_conv_desc*);
 int stat_rows(int64_t);
 int conv_dgrad_launch(const fsb_conv_desc*, const void*, int, const void*, const float*, int64_t, int64_t, void*, int, cudaStream_t);
 int conv_wgrad_launch(const fsb_conv_desc*, const void*, const void*, int, float*, int64_t, int64_t, int, float, cudaStream_t);
@@ -65,9 +64,9 @@ int fsb_conv_bn_act_train_fwd(const fsb_conv_desc* d, const void* x, const void*
   float* rows = vec + 6 * C;
   const bool direct = (c.flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(&c);
   const int64_t pixels = static_cast<int64_t>(d->N) * d->Ho * d->Wo;
-  int R = direct ? stat_rows(pixels) : (conv_tc2_supported(&c) ? conv_tc2_ctas(&c) : conv_tc_m_tiles(&c));
+  int R = direct ? stat_rows(pixels) : conv_tc_m_tiles(&c);
   int rc = direct ? conv_direct_launch(&c, x, wpacked, nullptr, nullptr, raw_f32, rows, st)
-                  : conv_tc_dispatch(&c, x, wpacked, nullptr, nullptr, raw_f32, rows, st);
+                  : conv_tc_launch(&c, x, wpacked, nullptr, nullptr, raw_f32, rows, st);
   if (rc) return rc;
   const int world = dp_world();
   const float* stats = rows;

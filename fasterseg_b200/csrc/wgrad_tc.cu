@@ -1,23 +1,23 @@
-// wgrad_tc.cu -- K7: convolution weight gradient on tcgen05 tensor cores.
+// wgrad_tc.cu -- K7: convolution weight gradient on Hopper tensor cores (wgmma, sm_90a).
 //
 //   dW[co, ci, r, s] = sum over output pixels p of  dy[p, co] * x[p * stride + (r, s) - pad, ci]
 //
 // Per filter tap this is a GEMM  D[M = co, N = ci] = A^T[M, K] * B[K, N]  with K = output pixels.  Both operands live in
-// memory as NHWC, i.e. pixel-major rows of channel-contiguous data, which is exactly the UMMA "MN-major" canonical layout:
+// memory as NHWC, i.e. pixel-major rows of channel-contiguous data, which is exactly the wgmma "MN-major" canonical layout:
 // a TMA box {64 channels, tw, th, 1} lands in shared memory as 128 rows (pixels = K) x 128 bytes (64 channels = M or N),
 // 128B-swizzled; 8-pixel groups are 1024 B apart (stride byte offset) and successive 64-channel blocks of the same pixels are
 // separate boxes, one tile (16 KB) apart (leading byte offset).  The x tile of tap (r,s) is the dy tile's pixel block
 // shifted by the tap (out-of-image pixels zero-filled by TMA; stride-2 convs read the matching parity plane), exactly like
 // the forward kernel's A operand.  No transposes, no im2col.
-// A CTA owns (co tile of 128, ci tile <= 256, tap, pixel chunk): the 128 x ci_tile fp32 accumulator sits in TMEM while it
-// walks its pixel chunk 128 pixels per pipeline stage; the epilogue adds the tile into the fp32 master-layout gradient with
-// atomics (pixel chunks of the same tile race benignly), scaled by 1/loss-scale.
+// A CTA owns (co tile of 128, ci tile of 64 or 128, tap, pixel chunk): warp 0 streams the pixel chunk 128 pixels per
+// pipeline stage, the warpgroup of warps 4-7 accumulates the 128 x ci_tile fp32 tile in registers (two m64 halves) and adds
+// it into the fp32 master-layout gradient with atomics (pixel chunks of the same tile race benignly), scaled by 1/loss-scale.
 #include "fsb_common.cuh"
 #include "fsb_internal.h"
 
 namespace fsb {
 
-constexpr int kWgThreads = 192;
+constexpr int kWgThreads = 256;
 constexpr int kWgMaxStages = 6;
 constexpr int kWgPix = 128;           // K per stage
 constexpr int kWgSub = kWgPix * 128;  // bytes of one [128 pixels x 64 channels] sub-tile
@@ -30,44 +30,27 @@ struct WgradTcParams {
   int tiles_w, tiles_h, n_img;  // pixel tiling of the OUTPUT map
   int tw, th;
   int Cout, Cin;
-  int co_tiles, ci_tiles, ci_tile;  // ci_tile: multiple of 64, <= 256
+  int co_tiles, ci_tiles;
   int chunks;                       // pixel-tile chunks (grid.y)
   int stages;
-  uint32_t tmem_cols;
   float inv_gscale;
   float* dw;
   long long so, si;
 };
 
-// K-major-in-memory-is-pixels: MN-major operand descriptor, 128B swizzle.
-//   LBO = distance between consecutive 64-element (128 B) blocks along M/N, SBO = distance between 8-row groups along K.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_f16_mn(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 15) | (1u << 16) | ((N >> 3) << 17) | ((M >> 4) << 24);  // both operands MN-major
-}
-
+template <int NT>  // ci tile: 64 or 128
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ WgradTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kWgMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kWgMaxStages];
-  __shared__ __align__(8) uint64_t tmem_full_bar;
-  __shared__ uint32_t tmem_base_smem;
 
   pdl_launch_dependents();
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int n_sub = p.ci_tile / 64;                   // x sub-tiles per stage
-  const uint32_t stage_bytes = static_cast<uint32_t>(2 + n_sub) * kWgSub;
+  constexpr int kSub = NT / 64;                     // x sub-tiles per stage
+  constexpr uint32_t kStageBytes = static_cast<uint32_t>(2 + kSub) * kWgSub;
 
   int b = blockIdx.x;
   const int co_t = b % p.co_tiles;
@@ -75,7 +58,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ WgradTcParams p) {
   const int ci_t = b % p.ci_tiles;
   b /= p.ci_tiles;
   const int tap = b;
-  const int co0 = co_t * 128, ci0 = ci_t * p.ci_tile;
+  const int co0 = co_t * 128, ci0 = ci_t * NT;
   const int total_tiles = p.tiles_w * p.tiles_h * p.n_img;
   const int per = (total_tiles + p.chunks - 1) / p.chunks;
   const int t_begin = blockIdx.y * per;
@@ -87,42 +70,33 @@ conv_wgrad_tc_kernel(const __grid_constant__ WgradTcParams p) {
     tma_prefetch_desc(&p.tmap_x[p.tap_map[tap]]);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);  // one arrival per warp of the MMA warpgroup
     }
-    mbar_init(&tmem_full_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 1) {
-    tmem_alloc(&tmem_base_smem, p.tmem_cols);
-    tmem_relinquish();
-  }
   pdl_wait();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = tmem_base_smem;
   if (n_iters <= 0) {
-    // nothing to do for this chunk (more chunks than tiles): fall through to the common teardown
+    // nothing to do for this chunk (more chunks than tiles)
   } else if (warp == 0) {
-    // converged warp, only the TMA issue under elect.sync (see conv_tc.cu: a divergent single-lane region turns every
-    // uniform-datapath instruction into an ELECT / R2UR / BRA.U.ANY waterfall)
+    // converged warp, only the TMA issue under elect.sync
     const CUtensorMap* mx = &p.tmap_x[p.tap_map[tap]];
     RingPos rp;
     uint8_t* st = smem;
     int tile_w = t_begin % p.tiles_w, tile_h = (t_begin / p.tiles_w) % p.tiles_h, img = t_begin / (p.tiles_w * p.tiles_h);
     for (int it = 0; it < n_iters; ++it) {
       const int w0 = tile_w * p.tw, h0 = tile_h * p.th;
-      mbar_wait(&empty_bar[rp.s], rp.phase ^ 1u);
+      mbar_wait_inline(&empty_bar[rp.s], rp.phase ^ 1u);
       if (elect_one()) {
-        mbar_arrive_expect_tx(&full_bar[rp.s], stage_bytes);
+        mbar_arrive_expect_tx(&full_bar[rp.s], kStageBytes);
         tma_load_4d(st, &p.tmap_dy, &full_bar[rp.s], co0, w0, h0, img);
         tma_load_4d(st + kWgSub, &p.tmap_dy, &full_bar[rp.s], co0 + 64, w0, h0, img);
-        for (int j = 0; j < n_sub; ++j)
+        for (int j = 0; j < kSub; ++j)
           tma_load_4d(st + static_cast<size_t>(2 + j) * kWgSub, mx, &full_bar[rp.s], ci0 + j * 64, w0 + p.tap_dw[tap],
                       h0 + p.tap_dh[tap], img);
       }
       __syncwarp();
-      st += stage_bytes;
+      st += kStageBytes;
       rp.advance(p.stages);
       if (rp.s == 0) st = smem;
       if (++tile_w == p.tiles_w) {   // next spatial tile without integer division
@@ -133,58 +107,48 @@ conv_wgrad_tc_kernel(const __grid_constant__ WgradTcParams p) {
         }
       }
     }
-  } else if (warp == 1) {
-    const uint32_t idesc = umma_idesc_f16_mn(128, static_cast<uint32_t>(p.ci_tile));
+  } else if (warp >= 4) {
+    const int tw = threadIdx.x - 128;  // thread index inside the warpgroup
+    float acc[2][NT / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) acc[h][i] = 0.f;
     const uint32_t s0 = smem_u32(smem);
     RingPos rp;
     uint32_t soff = 0;
+    int prev = -1;
     for (int it = 0; it < n_iters; ++it) {
-      mbar_wait(&full_bar[rp.s], rp.phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = s0 + soff;
-        const uint32_t sb = sa + 2 * kWgSub;
+      mbar_wait_inline(&full_bar[rp.s], rp.phase);
+      wgmma_fence();
+      const uint32_t sa = s0 + soff;
+      const uint32_t sb = sa + 2 * kWgSub;
 #pragma unroll
-        for (int k = 0; k < kWgPix / 16; ++k) {
-          // 16 pixels = two 8-row groups = 2048 B further down each sub-tile
-          const uint64_t da = umma_desc_mnmajor_sw128(sa + k * 2048, kWgSub);
-          const uint64_t db = umma_desc_mnmajor_sw128(sb + k * 2048, kWgSub);
-          umma_f16_ss(tmem_base, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[rp.s]);
-        if (it == n_iters - 1) umma_commit(&tmem_full_bar);
+      for (int k = 0; k < kWgPix / 16; ++k) {
+        // 16 pixels = two 8-row groups = 2048 B further down each sub-tile; co 0-63 / 64-127 are the two dy sub-tiles
+        const uint64_t db = wgmma_desc(sb + k * 2048, kWgSub, 1024, 128);
+        wgmma_f16<NT, 1>(acc[0], wgmma_desc(sa + k * 2048, kWgSub, 1024, 128), db);
+        wgmma_f16<NT, 1>(acc[1], wgmma_desc(sa + kWgSub + k * 2048, kWgSub, 1024, 128), db);
       }
-      __syncwarp();
-      soff += stage_bytes;
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous stage's MMAs have read their operands: hand that slot back to the producer
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = rp.s;
+      soff += kStageBytes;
       rp.advance(p.stages);
       if (rp.s == 0) soff = 0;
     }
-  } else {
-    const int q = warp & 3;
-    const int co = co0 + q * 32 + lane;
-    mbar_wait(&tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    for (int c = 0; c < p.ci_tile; c += 16) {
-      uint32_t v[16];
-      tmem_ld16(taddr + c, v);
-      tmem_ld_wait();
-      if (co < p.Cout) {
-        float* row = p.dw + static_cast<long long>(co) * p.so + tap;
+    wgmma_wait<0>();
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const int ci = ci0 + c + j;
-          if (ci < p.Cin) atomicAdd(row + static_cast<long long>(ci) * p.si, __uint_as_float(v[j]) * p.inv_gscale);
-        }
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < NT / 2; ++i) {
+        const int co = co0 + 64 * h + wgmma_row(tw, i), ci = ci0 + wgmma_col(tw, i);
+        if (co < p.Cout && ci < p.Cin)
+          atomicAdd(p.dw + static_cast<long long>(co) * p.so + tap + static_cast<long long>(ci) * p.si, acc[h][i] * p.inv_gscale);
       }
-    }
-    tc_fence_before();
   }
   __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, p.tmem_cols);
-  }
 }
 
 int encode_tiled_generic(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
@@ -216,15 +180,13 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
   p.Cin = d->Cin;
   p.co_tiles = (d->Cout + 127) / 128;
   const int ci64 = (d->Cin + 63) / 64 * 64;
-  p.ci_tile = ci64 > 256 ? (ci64 % 256 == 0 ? 256 : (ci64 % 192 == 0 ? 192 : (ci64 % 128 == 0 ? 128 : 64))) : ci64;
-  p.ci_tiles = (ci64 + p.ci_tile - 1) / p.ci_tile;
+  // ci tile of 64 or 128 channels: two m64 x ci_tile accumulators = at most 128 registers per thread
+  const int ci_tile = ci64 % 128 == 0 ? 128 : 64;
+  p.ci_tiles = ci64 / ci_tile;
   p.inv_gscale = 1.0f / gscale;
   p.dw = dw;
   p.so = so;
   p.si = si;
-  uint32_t cols = 32;
-  while (cols < static_cast<uint32_t>(p.ci_tile)) cols <<= 1;
-  p.tmem_cols = cols;
   const int total_tiles = p.tiles_w * p.tiles_h * d->N;
   const int fixed = p.co_tiles * p.ci_tiles * p.taps;
   int chunks = (sm_count() * 2 + fixed - 1) / fixed;
@@ -233,7 +195,7 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
   // writer and the fp32 accumulation order is fixed (slower: co_tiles * ci_tiles * taps CTAs only)
   if (chunks < 1 || opt(OPT_DETERMINISTIC) == 1) chunks = 1;
   p.chunks = chunks;
-  const size_t stage_bytes = static_cast<size_t>(2 + p.ci_tile / 64) * kWgSub;
+  const size_t stage_bytes = static_cast<size_t>(2 + ci_tile / 64) * kWgSub;
   int stages = static_cast<int>((192 * 1024) / stage_bytes);
   if (stages > kWgMaxStages) stages = kWgMaxStages;
   const int per = (total_tiles + chunks - 1) / chunks;
@@ -291,10 +253,12 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
         if (rc) return rc;
       }
   }
-  cudaError_t e;
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_wgrad_tc_kernel), 220 * 1024, "cudaFuncSetAttribute(conv_wgrad_tc)")) return rc;
+  const void* kernel = ci_tile == 128 ? reinterpret_cast<const void*>(conv_wgrad_tc_kernel<128>)
+                                      : reinterpret_cast<const void*>(conv_wgrad_tc_kernel<64>);
+  if (int rc = ensure_dyn_smem(kernel, 220 * 1024, "cudaFuncSetAttribute(conv_wgrad_tc)")) return rc;
   dim3 grid(static_cast<unsigned>(fixed), static_cast<unsigned>(chunks));
-  e = launch_kernel(conv_wgrad_tc_kernel, grid, dim3(kWgThreads), smem_bytes, stream, p);
+  const cudaError_t e = ci_tile == 128 ? launch_kernel(conv_wgrad_tc_kernel<128>, grid, dim3(kWgThreads), smem_bytes, stream, p)
+                                       : launch_kernel(conv_wgrad_tc_kernel<64>, grid, dim3(kWgThreads), smem_bytes, stream, p);
   if (e != cudaSuccess) return set_cuda_error(e, "conv_wgrad_tc launch");
   return FSB_OK;
 }

@@ -1,4 +1,4 @@
-"""Run an UNMODIFIED reference driver (search/train_search.py, train/train.py, latency/run_latency.py) on the B200 path.
+"""Run an UNMODIFIED reference driver (search/train_search.py, train/train.py, latency/run_latency.py) on the H100 (sm_90a) path.
 
     cd <FasterSeg>/search && python -m fasterseg_b200.launch train_search.py
     torchrun --nproc-per-node 8 -m fasterseg_b200.launch train_search.py        # data parallel

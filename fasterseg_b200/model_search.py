@@ -8,7 +8,7 @@ Same public surface as the reference (search/model_search.py:14-548): gumbel hel
 
 Organisation (ours): the trellis of cells is described once as a list of `_Node`s (layer, scale, which outputs of the
 previous layer feed it, which beta row mixes them); `forward` and `forward_latency` walk that list, and `_loss` runs a list
-of (architecture, width-mode) passes.  B200 side: NHWC fp16 activations; every conv+BN+ReLU is one fused tcgen05 unit (train
+of (architecture, width-mode) passes.  GPU side: NHWC fp16 activations; every conv+BN+ReLU is one fused wgmma unit (train
 mode: conv with fused statistics, finalize, apply); the `result + op(x) * w * r0 * r1` accumulation over the five
 primitives and the beta-weighted mix of the two cell invocations are single weighted-sum kernels (K5) whose backward also
 yields the scalar gradients of alphas / betas / ratios; logits leave as NCHW fp32 through one layout kernel.

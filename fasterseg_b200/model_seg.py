@@ -8,7 +8,7 @@ branch_groups, cells, ch_16 ...`) and every parameter name (`stem.0.conv.0.weigh
 Organisation (ours): `build_structure` compiles the decoded branches into a flat *schedule* -- one `_CellStep` per distinct
 cell in execution order (which branches share it, where a stream fork happens) plus one `_Tail` per branch (its
 arm / refine chain towards the 1/8 feature) -- and `forward`, `predict_labels` and `forward_latency` are interpreters of
-that schedule.  B200 side: NHWC fp16 activations, each conv+BN+ReLU one fused tcgen05 kernel, the torch.cat call sites
+that schedule.  GPU side: NHWC fp16 activations, each conv+BN+ReLU one fused wgmma kernel, the torch.cat call sites
 (:307,312,319,331) replaced by producers writing into channel slices of one buffer, independent branches on their own CUDA
 streams inside one CUDA graph, the final x8 upsample as one kernel writing NCHW logits (or, via `predict_labels`, a fused
 upsample+argmax that never materialises them).

@@ -5,7 +5,7 @@ API kept from search/operations.py:42-552: class names, constructor signatures, 
 (`C_in, C_out, stride, ratio, slimmable, width_mult_list`), registries `OPS / OPS_name / OPS_Class`
 and the parameter names that make up the checkpoint format (`conv1.weight`, `bn1.bn.{i}.*`, `conv.0.weight` ...).
 
-Execution differs completely: activations are NHWC fp16, each conv+BN(+ReLU) is one fused tcgen05
+Execution differs completely: activations are NHWC fp16, each conv+BN(+ReLU) is one fused wgmma
 implicit-GEMM kernel (`engine.conv_bn_act`), the "zoomed" ops run bilinear down / up as vectorised resize
 kernels with the trailing ReLU fused into the upsample, and `out=` lets a caller have the result written
 straight into a channel slice of a concat buffer.

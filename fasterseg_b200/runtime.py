@@ -1,6 +1,6 @@
 """Inference runtime: CUDA-graph capture of a whole network forward and a host<->device pipeline.
 
-The reference launches ~70 framework kernels per student frame from Python (train/model_seg.py:337-366); at B200
+The reference launches ~70 framework kernels per student frame from Python (train/model_seg.py:337-366); at H100
 speeds the frame is launch-bound long before it is HBM- or tensor-bound (SURVEY section 8d), so the whole forward is
 captured once into a CUDA graph and replayed.  `InferencePipeline` overlaps the H2D copy of frame i+1, the graph
 replay of frame i and the D2H copy of frame i-1 on three streams.

@@ -1,4 +1,4 @@
-/* fsb200.h -- C ABI of libfsb200.so: B200 (sm_100a) kernels for the FasterSeg conv hot path.
+/* fsb200.h -- C ABI of libfsb200.so: H100 (sm_90a) kernels for the FasterSeg conv hot path.
  *
  * The reference (VITA-Group/FasterSeg) has no FFI of its own: its hot path bottoms out in
  * torch.nn.functional calls (SURVEY.md section 8b).  Each entry point below therefore cites the
@@ -97,11 +97,13 @@ const char* fsb_last_error_string(void);
 int fsb_device_info(int* sm_count, int* cc_major, int* cc_minor);
 
 /* Programmatic dependent launch between consecutive kernels of this library (default on; env FSB_PDL=0 disables).
- * With it a kernel's prologue (barrier init, TMEM allocation, descriptor prefetch) overlaps its predecessor's tail. */
+ * With it a kernel's prologue (barrier init, descriptor prefetch) overlaps its predecessor's tail. */
 int fsb_set_pdl(int enabled);
-/* Tuning / validation switches, named like their environment variables (FSB_CONV_TC2, FSB_TC2_R, FSB_NO_TMA_STORE,
- * FSB_DGRAD_S2_DIRECT, FSB_WGRAD_TC, FSB_CONV_PERSIST, FSB_PERSIST_OCC, FSB_PERSIST_STAGES, FSB_UPSAMPLE_V2,
- * FSB_DETERMINISTIC, FSB_CONV_TC3).  The environment is read once at first use; value -1 = unset. */
+/* Tuning / validation switches, named like their environment variables (FSB_CONV_TC2: row-strip mode of the conv kernel,
+ * FSB_NO_TMA_STORE, FSB_DGRAD_S2_DIRECT, FSB_WGRAD_TC, FSB_UPSAMPLE_V2, FSB_DETERMINISTIC, FSB_CONV_NTILE_MIN).  The names of
+ * switches of earlier kernel variants (FSB_TC2_R, FSB_TC2_ASTAGES, FSB_CONV_TC3..5, FSB_CONV_PERSIST, FSB_PERSIST_OCC,
+ * FSB_PERSIST_STAGES, FSB_CONV_KSPLIT) are still accepted and have no effect.  The environment is read once at first use;
+ * value -1 = unset. */
 int fsb_set_option(const char* name, int value);
 int fsb_get_option(const char* name);
 
@@ -127,12 +129,13 @@ int fsb_bn_fold(int C, const float* gamma, const float* beta, const float* mean,
  *                      * w[co,ci,r,s]) * scale[co] + shift[co] )
  * x, y: fp16 NHWC with the strides in `d`; wpacked from fsb_pack_conv_weight; scale/shift fp32[Cout] or NULL;
  * stats fp32[2*Cout] (only with FSB_CONV_STATS; caller zeroes it).
- * Dense 3x3 / 1x1 contractions run as an im2col-free implicit GEMM on tcgen05 tensor cores with TMA-staged
+ * Dense 3x3 / 1x1 contractions run as an im2col-free implicit GEMM on the wgmma tensor cores with TMA-staged
  * NHWC tiles; Cin < 16 (the RGB stem) and FSB_CONV_FORCE_DIRECT use the CUDA-core direct kernel. */
 int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
                  void* y, float* stats, void* stream);
-/* which kernel fsb_conv_fwd dispatches for `d` (y: the output pointer, its alignment matters): 0 = CUDA-core direct, 1 = per-tap
- * tcgen05 (conv_tc), 2 = row-strip (conv_tc2), 3 = channel-major 128x256 (conv_tc3); negative = invalid descriptor */
+/* which kernel fsb_conv_fwd dispatches for `d`: 0 = CUDA-core direct, 1 = per-tap wgmma (conv_tc), 2 = conv_tc in row-strip
+ * mode (one input window per channel chunk, taps as descriptor offsets); negative = invalid descriptor.  y and with_stats are
+ * accepted for compatibility and do not change the choice. */
 int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats);
 /* number of partial statistic rows fsb_conv_fwd writes for `d` with FSB_CONV_STATS (depends on the kernel it dispatches):
  * stats must hold rows * 2 * SC floats; every row's entries of this conv's channels are written (no zeroing needed). */
@@ -240,7 +243,7 @@ int fsb_relu_bwd(int64_t pixels, int C, const void* dy, int dy_cstride, const vo
 /* conv data gradient (autograd of F.conv2d wrt input): dx[n,hi,wi,ci] = sum_{r,s,co} dy[n,ho,wo,co] * w[co,ci,r,s] over the
  * (ho,wo,r,s) with ho*stride + r - pad + off_h == hi (same for w).  `d` describes the FORWARD conv (x: N,H,W,Cin ...);
  * dy has d->Ho x d->Wo x Cout with pixel stride dy_cstride; dx has H x W x Cin with pixel stride dx_cstride.
- * w: fp32 OIHW master weight with strides like fsb_pack_conv_weight.  Stride-1 convs run on the tcgen05 kernel with
+ * w: fp32 OIHW master weight with strides like fsb_pack_conv_weight.  Stride-1 convs run on the tensor-core kernel with
  * a transposed/rotated weight pack (wpacked_t from fsb_pack_conv_weight_dgrad); others use the direct kernel. */
 size_t fsb_conv_packed_dgrad_bytes(const fsb_conv_desc* d);
 int fsb_pack_conv_weight_dgrad(const fsb_conv_desc* d, const float* w, int64_t w_stride_o, int64_t w_stride_i, void* packed_t,

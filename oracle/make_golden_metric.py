@@ -47,6 +47,21 @@ def normalize_inputs(name):
     return rs.randint(0, 256, size=shape).astype(np.uint8), np.array(mean), np.array(std)
 
 
+def hist_info_restated(n_cl, pred, gt):
+    """oracle restatement of tools/seg_opr/metric.py:7-15 hist_info: confusion matrix (row = ground truth, column = prediction)
+    over the pixels whose ground truth lies in [0, n_cl), their count, and how many of them are predicted correctly"""
+    valid = (gt >= 0) & (gt < n_cl)
+    g, p = gt[valid].astype(np.int64), pred[valid].astype(np.int64)
+    hist = np.bincount(n_cl * g + p, minlength=n_cl * n_cl).reshape(n_cl, n_cl)
+    return hist, int(valid.sum()), int((p == g).sum())
+
+
+def normalize_restated(img, mean, std):
+    """oracle restatement of tools/utils/img_utils.py:179-185 normalize, same dtypes: uint8 -> float32 / 255, then the float64
+    mean and std per channel"""
+    return (img.astype(np.float32) / np.float32(255) - mean) / std
+
+
 def _load(path, name):
     spec = importlib.util.spec_from_file_location(name, path)
     mod = importlib.util.module_from_spec(spec)

@@ -1,10 +1,9 @@
 """TEST INFRASTRUCTURE ONLY -- loader for the *unmodified* reference (VITA-Group/FasterSeg).
 
-This module exists so that `oracle/make_golden.py` (run in the build container, where
-`/root/reference` is mounted read-only) can import the reference's own Python modules,
-run them on CPU fp32 and write golden vectors to `tests/golden/`.  Nothing in the product
-path (`fasterseg_b200/`) imports it, and nothing on the GPU box can use it
-(`/root/reference` does not exist there).
+This module exists so that `oracle/make_golden*.py` (run where a checkout of the reference is
+available) can import the reference's own Python modules, run them on CPU fp32 and write golden
+vectors to `tests/golden/`.  Nothing in the product path (`fasterseg_b200/`) imports it, and no
+test depends on the reference tree: the tests read the stored goldens.
 
 Why a harness is needed (SURVEY.md section 5 "compat list", section 8c):
   * `operations.py:12-17` computes `root_dir = abs_dir[:abs_dir.index('FasterSeg')...]`
@@ -25,11 +24,13 @@ import sys
 import tempfile
 import types
 
-# The mounted tree, or -- on the GPU box, where /root/reference does not exist -- the verbatim copy that __graft_entry__.build() drops
-# into the git-ignored oracle/_ref/FasterSeg (build output, never committed; it only exists so that `bench.py --impl reference` and the
-# cpu_baseline leg can time the UNMODIFIED reference on the box's host cores).
+# Where the reference checkout lives: $FASTERSEG_REFERENCE, else a directory `reference` next to this repository, else the verbatim
+# copy that install_local_copy() (called by __graft_entry__.build()) keeps in the git-ignored oracle/_ref/FasterSeg, so that
+# `bench.py --impl reference` and the cpu_baseline leg can time the UNMODIFIED reference on machines without the checkout.
 _LOCAL_COPY = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref", "FasterSeg")
-REFERENCE_ROOT = os.environ.get("FASTERSEG_REFERENCE") or ("/root/reference" if os.path.isdir("/root/reference/search") else _LOCAL_COPY)
+_SIBLING = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "..", "reference")
+REFERENCE_ROOT = os.environ.get("FASTERSEG_REFERENCE") or (os.path.normpath(_SIBLING) if os.path.isdir(os.path.join(_SIBLING, "search"))
+                                                          else _LOCAL_COPY)
 _SCRATCH = None
 _REF_MODULE_NAMES = (
     "operations", "slimmable_ops", "seg_oprs", "model_seg", "model_search", "genotypes",
@@ -83,6 +84,14 @@ def _install_stubs() -> None:
 
         tb.SummaryWriter = SummaryWriter
         sys.modules["tensorboardX"] = tb
+
+
+def install_local_copy() -> None:
+    """Copy the reference checkout (without images) to oracle/_ref/FasterSeg once, if a checkout is available."""
+    if REFERENCE_ROOT == _LOCAL_COPY or not reference_available() or os.path.isdir(os.path.join(_LOCAL_COPY, "search")):
+        return
+    os.makedirs(os.path.dirname(_LOCAL_COPY), exist_ok=True)
+    shutil.copytree(REFERENCE_ROOT, _LOCAL_COPY, ignore=shutil.ignore_patterns("images", "*.png", "*.jpg", "*.gif", ".git"))
 
 
 def scratch_copy() -> str:

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -34,8 +34,3 @@ def lib_option():
     yield setter
     for name, old in reversed(saved):
         _lib.set_option(name, old)
-
-
-@pytest.fixture
-def tc2_forced(lib_option):
-    return lambda: lib_option("FSB_CONV_TC2", 2)

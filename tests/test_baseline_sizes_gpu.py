@@ -1,7 +1,7 @@
 """GPU parity at the sizes BASELINE.json's configs name (round 1 only covered reduced sizes), against digests of the UNMODIFIED
 reference produced by oracle/make_golden_baseline.py (tests/golden/baseline_sizes.*):
   C2  student arch_1 eval forward 1 x 3 x 1024 x 2048 -- the benchmarked configuration; this input size is what sends the big layers
-      through the channel-major (conv_tc3) and row-strip (conv_tc2) kernels and the N-split heuristics of conv_tc;
+      through the row-strip and per-tap modes and the N-split heuristics of conv_tc;
   C3  16-layer supernet pretrain `_loss` + backward at 3 x 3 x 256 x 512 (captured passes, fasterseg_b200/graphed.py);
   C5  16-layer supernet search `_loss` + backward at 2 x 3 x 224 x 448.
 Label maps: "bit-exact argmax" cannot hold literally for an fp16-storage pipeline against an fp32 one wherever two logits are

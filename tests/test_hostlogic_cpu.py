@@ -314,18 +314,23 @@ def test_normalisation_table_matches_the_reference_normalize(name):
 
 
 def test_metric_goldens_are_what_the_live_reference_computes():
+    """tests/golden/metric.json holds the reference's hist_info / normalize outputs on inputs that the tests regenerate from seeds:
+    the regenerated inputs must still produce exactly those outputs -- through the oracle restatement of the two functions always,
+    and through the reference's own functions wherever a reference checkout is available (oracle/ref_harness.py)"""
     from oracle import make_golden_metric as mk
     from oracle import ref_harness
-    if not ref_harness.reference_available():
-        pytest.skip("reference tree not mounted")
-    metric, normalize = mk.reference_modules()
+    impls = [(mk.hist_info_restated, mk.normalize_restated)]
+    if ref_harness.reference_available():
+        metric, normalize = mk.reference_modules()
+        impls.append((metric.hist_info, normalize))
     gold = H.load_json("metric.json")
-    for name in mk.CASES:
-        n_cl, pred, gt = mk.metric_inputs(name)
-        hist, labeled, correct = metric.hist_info(n_cl, pred, gt)
-        assert hist.tolist() == gold["metric"][name]["hist"] and int(labeled) == gold["metric"][name]["labeled"]
-        assert int(correct) == gold["metric"][name]["correct"]
-    for name in mk.NORMALIZE_CASES:
-        img, mean, std = mk.normalize_inputs(name)
-        got = np.stack([normalize(im, mean, std) for im in img]).astype(np.float32)
-        assert got.reshape(-1)[:12].tolist() == gold["normalize"][name]["first"]
+    for hist_info, normalize in impls:
+        for name in mk.CASES:
+            n_cl, pred, gt = mk.metric_inputs(name)
+            hist, labeled, correct = hist_info(n_cl, pred, gt)
+            assert hist.tolist() == gold["metric"][name]["hist"] and int(labeled) == gold["metric"][name]["labeled"]
+            assert int(correct) == gold["metric"][name]["correct"]
+        for name in mk.NORMALIZE_CASES:
+            img, mean, std = mk.normalize_inputs(name)
+            got = np.stack([normalize(im, mean, std) for im in img]).astype(np.float32)
+            assert got.reshape(-1)[:12].tolist() == gold["normalize"][name]["first"]

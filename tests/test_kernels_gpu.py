@@ -58,7 +58,7 @@ CONV_CASES = [
     (1, 192, 128, 3, 1, 32, 64),
     (3, 80, 48, 1, 1, 6, 10),
     (1, 16, 16, 3, 1, 8, 8),
-    # wide maps -> row-strip kernel (conv_tc2.cu): R rows x 128 columns per CTA, halo rows read once
+    # wide maps: many spatial tiles, ragged last tiles
     (1, 64, 64, 3, 1, 20, 256),
     (2, 32, 32, 3, 1, 9, 130),
     (1, 128, 128, 3, 1, 16, 128),
@@ -71,10 +71,8 @@ CONV_CASES = [
 
 @pytest.mark.parametrize("case", CONV_CASES)
 @pytest.mark.parametrize("direct", [False, True])
-def test_conv_bn_relu_matches_oracle(case, direct, tc2_forced):
+def test_conv_bn_relu_matches_oracle(case, direct):
     F_ = _F()
-    if case[6] >= 96 and case[3] == 3 and case[4] == 1:
-        tc2_forced()  # exercise the row-strip kernel on every wide 3x3 case, not only where it is faster
     N, Cin, Cout, k, stride, Hh, Ww = case
     seed = hash(case) % 100000
     x = _rand((N, Cin, Hh, Ww), seed).half().float()
@@ -90,23 +88,45 @@ def test_conv_bn_relu_matches_oracle(case, direct, tc2_forced):
     _close(y.float().cpu(), ref)
 
 
-# channel-major 128 x 256 kernel (conv_tc3.cu): Cin % 64 == 0, Cout % 64 == 0, Cout >= 128; forced on (it is only dispatched on
-# maps >= 12 288 pixels by default)
-TC3_CASES = [
+# conv_tc written into a channel slice of a wider buffer (zero-copy concat: the TMA store must respect offset and stride).
+# Cases: ragged tiles, batch > 1, 1x1 and stride 2, Wo < 16 (8 x 16 tiles), every N-tile width (Cout 16 .. 256, split into 128-wide
+# tiles), 1 .. 4 channel chunks, single-row images, maps with far more tiles than SMs.
+SLICE_CASES = [
     # N, Cin, Cout, k, stride, H, W
-    (1, 128, 128, 3, 1, 32, 64),     # heads8-like
-    (1, 192, 128, 3, 1, 24, 40),     # refines32.0-like, ragged tiles (24 x 40 is not a multiple of 8 x 32)
-    (2, 64, 192, 3, 1, 9, 21),       # two M tiles (128 + 64), odd sizes, batch 2
-    (1, 128, 128, 1, 1, 16, 48),     # 1x1 (ffm)
-    (1, 64, 128, 3, 2, 34, 50),      # stride 2: parity planes
-    (1, 256, 256, 3, 1, 8, 12),      # Wo < 16 -> 8 x 32 tiles, 2 M tiles, 4 k-chunks
+    (1, 128, 128, 3, 1, 32, 64),
+    (1, 192, 128, 3, 1, 24, 40),
+    (2, 64, 192, 3, 1, 9, 21),
+    (1, 128, 128, 1, 1, 16, 48),
+    (1, 64, 128, 3, 2, 34, 50),
+    (1, 256, 256, 3, 1, 8, 12),
+    (1, 128, 128, 3, 1, 16, 256),
+    (1, 64, 64, 3, 1, 40, 256),
+    (1, 64, 64, 3, 1, 600, 128),
+    (1, 64, 64, 3, 1, 1500, 128),
+    (1, 128, 128, 3, 1, 700, 128),
+    (2, 64, 128, 3, 1, 9, 200),
+    (1, 64, 64, 3, 1, 7, 130),
+    (3, 64, 64, 3, 1, 5, 128),
+    (1, 192, 128, 3, 1, 12, 128),
+    (1, 128, 256, 3, 1, 6, 128),
+    (1, 64, 192, 3, 1, 10, 256),
+    (1, 64, 64, 3, 1, 24, 256),
+    (1, 64, 32, 3, 1, 33, 100),
+    (2, 64, 64, 3, 1, 7, 130),
+    (1, 128, 32, 3, 1, 9, 64),
+    (1, 128, 48, 3, 1, 5, 37),
+    (1, 256, 16, 3, 1, 3, 500),
+    (1, 192, 32, 3, 1, 6, 90),
+    (1, 64, 64, 3, 1, 1, 300),
+    (3, 64, 64, 3, 1, 160, 128),
 ]
 
 
-@pytest.mark.parametrize("case", TC3_CASES)
-def test_conv_tc3_channel_major_kernel(case, lib_option):
+@pytest.mark.parametrize("case", SLICE_CASES)
+def test_conv_tc_into_channel_slice(case, lib_option):
     F_ = _F()
-    lib_option("FSB_CONV_TC3", 2)
+    from fasterseg_b200 import _lib
+    import ctypes as C
     N, Cin, Cout, k, stride, Hh, Ww = case
     seed = hash(case) % 100000
     x = _rand((N, Cin, Hh, Ww), seed).half().float()
@@ -116,116 +136,29 @@ def test_conv_tc3_channel_major_kernel(case, lib_option):
     pad = 1 if k == 3 else 0
     ref = torch.relu(orc.conv2d(x, w, None, stride, pad) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
     wp = F_.pack_conv_weight(w.cuda(), Cin, Cout, k)
-    # into a channel slice of a wider buffer: the TMA store must respect offset and stride (zero-copy concat)
     Ho, Wo = ref.shape[2], ref.shape[3]
     cat = F_.empty_nhwc(N, Cout + 64, Ho, Wo, "cuda")
     cat.fill_(7.0)
-    y = F_.conv_fwd(_nhwc(x), wp, Cout, k, stride, pad, scale.cuda(), shift.cuda(), relu=True, out=cat[:, 32:32 + Cout])
+    out = cat[:, 32:32 + Cout]
+    d = _lib.ConvDesc(N, Hh, Ww, Cin, Cout, k, stride, pad, 1, 0, 0, Ho, Wo, Cin, Cout + 64, _lib.FSB_CONV_RELU | _lib.FSB_CONV_AFFINE)
+    assert _lib.lib().fsb_conv_kernel_id(C.byref(d), C.c_void_p(out.data_ptr()), 0) == 1, "case does not reach the tensor-core kernel"
+    y = F_.conv_fwd(_nhwc(x), wp, Cout, k, stride, pad, scale.cuda(), shift.cuda(), relu=True, out=out)
     torch.cuda.synchronize()
     _close(y.float().cpu(), ref)
     assert float((cat[:, :32] - 7.0).abs().max()) == 0.0 and float((cat[:, 32 + Cout:] - 7.0).abs().max()) == 0.0
-    # bit-identical to the per-tap kernel? no -- different accumulation order; but no epilogue / no relu must agree closely
-    lib_option("FSB_CONV_TC3", 0)
+    # the same kernel into a dense tensor: the destination layout must not change a single bit
     y0 = F_.conv_fwd(_nhwc(x), wp, Cout, k, stride, pad, scale.cuda(), shift.cuda(), relu=True)
     torch.cuda.synchronize()
-    assert float((y0.float() - y.float()).abs().max()) <= 2e-3 * float(ref.abs().max())
-
-
-# CTA-pair row-rolling kernel (conv_tc4.cu): 3x3 stride-1, Cin % 64 == 0, Cout % 64 == 0, >= 96 output columns; forced on so the
-# small cases below reach it.  The cases cover: resident weights (64->64) and streamed weights with lagged row pairs
-# (128->128), recycled input-row slots (many rows per CTA), ragged strips (Wo % 128 != 0), an odd job count (inert
-# partner CTA), batch > 1, Cin = 192 (3 channel chunks), Cout = 192 / 256.
-TC4_CASES = [
-    # N, Cin, Cout, H, W
-    (1, 128, 128, 16, 256),    # heads8-like: streamed weights, R rows in lagged pairs
-    (1, 64, 64, 40, 256),      # stem.1.conv2-like: resident weights
-    (1, 64, 64, 600, 128),     # R = 5 rows per CTA at 148 SMs: every input row loaded once, 120 jobs
-    (1, 64, 64, 1500, 128),    # R = 11 > row slots: the input-row ring recycles
-    (1, 128, 128, 700, 128),   # streamed weights, R = 5 (groups of 2 + a single row), recycled rows
-    (2, 64, 128, 9, 200),      # ragged strip (200 = 128 + 72), batch 2, 18 x 2 = 36 jobs
-    (1, 64, 64, 7, 130),       # 2 strips x 7 rows = 14 jobs, second strip 2 columns wide
-    (3, 64, 64, 5, 128),       # 15 jobs: odd -> one inert partner CTA
-    (1, 192, 128, 12, 128),    # 3 channel chunks
-    (1, 128, 256, 6, 128),     # N = 256 (one accumulator), 2 channel chunks
-    (1, 64, 192, 10, 256),     # N = 192
-]
-
-
-@pytest.mark.parametrize("case", TC4_CASES)
-def test_conv_tc4_cta_pair_kernel(case, lib_option):
-    F_ = _F()
-    from fasterseg_b200 import _lib
-    import ctypes as C
-    lib_option("FSB_CONV_TC4", 2)
-    lib_option("FSB_CONV_TC5", 0)   # the tap-concatenated kernel is dispatched first where both apply
-    N, Cin, Cout, Hh, Ww = case
-    seed = hash(case) % 100000
-    x = _rand((N, Cin, Hh, Ww), seed).half().float()
-    w = (_rand((Cout, Cin, 3, 3), seed + 1) * (2.0 / (Cin * 9)) ** 0.5).half().float()
-    scale = torch.from_numpy(np.random.RandomState(seed + 2).uniform(0.5, 1.5, Cout).astype(np.float32))
-    shift = _rand((Cout,), seed + 3, 0.2)
-    ref = torch.relu(orc.conv2d(x, w, None, 1, 1) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
-    wp = F_.pack_conv_weight(w.cuda(), Cin, Cout, 3)
-    cat = F_.empty_nhwc(N, Cout + 64, Hh, Ww, "cuda")
-    cat.fill_(7.0)
-    out = cat[:, 32:32 + Cout]
-    d = _lib.ConvDesc(N, Hh, Ww, Cin, Cout, 3, 1, 1, 1, 0, 0, Hh, Ww, Cin, Cout + 64, _lib.FSB_CONV_RELU | _lib.FSB_CONV_AFFINE)
-    assert _lib.lib().fsb_conv_kernel_id(C.byref(d), C.c_void_p(out.data_ptr()), 0) == 4, "case does not reach the pair kernel"
-    y = F_.conv_fwd(_nhwc(x), wp, Cout, 3, 1, 1, scale.cuda(), shift.cuda(), relu=True, out=out)
-    torch.cuda.synchronize()
-    _close(y.float().cpu(), ref)
-    assert float((cat[:, :32] - 7.0).abs().max()) == 0.0 and float((cat[:, 32 + Cout:] - 7.0).abs().max()) == 0.0
-    lib_option("FSB_CONV_TC4", 0)
-    y0 = F_.conv_fwd(_nhwc(x), wp, Cout, 3, 1, 1, scale.cuda(), shift.cuda(), relu=True)
-    torch.cuda.synchronize()
-    assert float((y0.float() - y.float()).abs().max()) <= 2e-3 * float(ref.abs().max())
-
-
-# tap-concatenated kernel (conv_tc5.cu): 3x3 stride-1, Cin % 64 == 0, Cout in {16, 32, 48, 64}; flattened-pixel tiles of 126 outputs.
-# Cases: tiles crossing image rows (W not a multiple of 126), W smaller than a tile (several rows per tile), single-row images,
-# batch > 1 (tile -> image mapping), 1..4 channel chunks, every supported Cout, more tiles than SMs (persistent loop + both TMEM
-# accumulators reused), zero-copy concat destination.
-TC5_CASES = [
-    # N, Cin, Cout, H, W
-    (1, 64, 64, 24, 256),      # stem.1.conv2-like
-    (1, 64, 32, 33, 100),      # cell0.conv1-like, W < tile
-    (2, 64, 64, 7, 130),       # batch 2, ragged
-    (1, 128, 32, 9, 64),       # two channel chunks, 1.9 rows per tile
-    (1, 128, 48, 5, 37),       # Cout = 48, odd sizes
-    (1, 256, 16, 3, 500),      # four chunks, Cout = 16
-    (1, 192, 32, 6, 90),       # three chunks
-    (1, 64, 64, 1, 300),       # a single image row (top and bottom padding in every tile)
-    (3, 64, 64, 160, 128),     # 3 x 163 = 489 tiles > 148 SMs: persistent walk, accumulator ring
-]
-
-
-@pytest.mark.parametrize("case", TC5_CASES)
-def test_conv_tc5_tap_concatenated_kernel(case, lib_option):
-    F_ = _F()
-    from fasterseg_b200 import _lib
-    import ctypes as C
-    lib_option("FSB_CONV_TC5", 2)
-    N, Cin, Cout, Hh, Ww = case
-    seed = hash(case) % 100000
-    x = _rand((N, Cin, Hh, Ww), seed).half().float()
-    w = (_rand((Cout, Cin, 3, 3), seed + 1) * (2.0 / (Cin * 9)) ** 0.5).half().float()
-    scale = torch.from_numpy(np.random.RandomState(seed + 2).uniform(0.5, 1.5, Cout).astype(np.float32))
-    shift = _rand((Cout,), seed + 3, 0.2)
-    ref = torch.relu(orc.conv2d(x, w, None, 1, 1) * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1))
-    wp = F_.pack_conv_weight(w.cuda(), Cin, Cout, 3)
-    cat = F_.empty_nhwc(N, Cout + 64, Hh, Ww, "cuda")
-    cat.fill_(7.0)
-    out = cat[:, 32:32 + Cout]
-    d = _lib.ConvDesc(N, Hh, Ww, Cin, Cout, 3, 1, 1, 1, 0, 0, Hh, Ww, Cin, Cout + 64, _lib.FSB_CONV_RELU | _lib.FSB_CONV_AFFINE)
-    assert _lib.lib().fsb_conv_kernel_id(C.byref(d), C.c_void_p(out.data_ptr()), 0) == 5, "case does not reach the tap-concatenated kernel"
-    y = F_.conv_fwd(_nhwc(x), wp, Cout, 3, 1, 1, scale.cuda(), shift.cuda(), relu=True, out=out)
-    torch.cuda.synchronize()
-    _close(y.float().cpu(), ref)
-    assert float((cat[:, :32] - 7.0).abs().max()) == 0.0 and float((cat[:, 32 + Cout:] - 7.0).abs().max()) == 0.0
-    lib_option("FSB_CONV_TC5", 0)
-    y0 = F_.conv_fwd(_nhwc(x), wp, Cout, 3, 1, 1, scale.cuda(), shift.cuda(), relu=True)
-    torch.cuda.synchronize()
-    assert float((y0.float() - y.float()).abs().max()) <= 2e-3 * float(ref.abs().max())
+    assert float((y0.float() - y.float()).abs().max()) == 0.0
+    if k == 3 and stride == 1 and Cin % 64 == 0:
+        # the row-strip mode (FSB_CONV_TC2=2: one input window per channel chunk, taps as descriptor offsets) on the same case
+        lib_option("FSB_CONV_TC2", 2)
+        assert _lib.lib().fsb_conv_kernel_id(C.byref(d), C.c_void_p(out.data_ptr()), 0) == 2
+        cat.fill_(7.0)
+        ys = F_.conv_fwd(_nhwc(x), wp, Cout, k, stride, pad, scale.cuda(), shift.cuda(), relu=True, out=out)
+        torch.cuda.synchronize()
+        _close(ys.float().cpu(), ref)
+        assert float((cat[:, :32] - 7.0).abs().max()) == 0.0 and float((cat[:, 32 + Cout:] - 7.0).abs().max()) == 0.0
 
 
 def test_statistics_are_bit_reproducible():

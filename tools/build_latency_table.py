@@ -9,7 +9,7 @@ fusion and heads for Fch in {8, 12} at 1024x2048 -- builds each operator from `f
 times it on the current device (CUDA events, warm-up + fixed iterations; `--protocol reference` uses the reference's
 doubling protocol of tools/utils/darts_utils.py:182-223 instead, ~7 s per entry).
 
-  python tools/build_latency_table.py --out latency_lookup_table.npy            # ~1 min on a B200
+  python tools/build_latency_table.py --out latency_lookup_table.npy            # one pass over the 667 operator shapes
   python tools/build_latency_table.py --list                                    # print the keys only (no GPU needed)
 
 `table_keys()` is checked on the build machine against the key set of the reference's shipped table
@@ -118,7 +118,7 @@ def time_module(module, shape, protocol="fast", iters=30):
         return compute_latency_ms(module, shape)
     module = module.cuda().eval()
     x = torch.randn(*shape, device="cuda")
-    flush = torch.empty(160 << 20, dtype=torch.uint8, device="cuda")     # > 126 MB L2
+    flush = torch.empty(160 << 20, dtype=torch.uint8, device="cuda")     # > 50 MB L2
     start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     total = 0.0
     with torch.no_grad():

@@ -22,7 +22,7 @@ from fasterseg_b200._lib import ConvDesc  # noqa: E402
 
 CALLS = {}
 WORK = {"flops": 0.0, "bytes": 0.0, "roof_s": 0.0}   # algorithmic work of the launches the stubs stand for
-PEAK_TFLOPS, PEAK_GBS = 1694.0, 6568.7               # MEASURED_PEAKS.json of this pool's B200s
+PEAK_TFLOPS, PEAK_GBS = 989.0, 3350.0                # H100 SXM data sheet (dense FP16, HBM3), not measured
 
 
 def _count(name):
