@@ -9,6 +9,8 @@
 //             tap-shifted coordinate; out-of-image rows/cols and channel tails are zero-filled by TMA, so
 //             padding costs nothing and no im2col buffer exists.  Stride-2 convs address one of four
 //             parity planes of the input (each its own tensor map), which keeps every box dense.
+//             3x3 stride-1 convs run in window mode instead (K walked as (64-channel chunk, tap)): one halo window of
+//             the input per chunk, the nine taps read from it through shifted descriptors (see below).
 //   B tile  : packed fp16 weights [tap][Npad][Kpad] (K-major), one TMA box {BK, NT, 1}.
 //   D       : fp32 accumulator in the registers of one warpgroup (two m64 halves of the 128-pixel tile, NT <= 128
 //             columns each: at most 128 accumulator registers per thread).
@@ -41,6 +43,14 @@ struct ConvTcParams {
   int Ho, Wo;
   int tiles_w, tiles_h;
   int tw, th;
+  // window mode only (see conv_tc_kernel): window = win_rows x win_pitch input pixels of 128 B; A row (half h, 8-row group g,
+  // row i) of tap (r,s) is window pixel (r * win_pitch + s) + h * win_half + g * win_sbo / 128 + i, which is tile pixel
+  // h * m_half + g * m_grp + i
+  int win_pitch, win_rows;
+  int win_sbo;     // bytes between 8-pixel groups (wgmma stride byte offset)
+  int win_half;    // pixels between the two m64 halves
+  int win_stride;  // bytes per window buffer (1024-aligned)
+  int m_half, m_grp;
   int Cout;
   int stages;
   int y_cstride;
@@ -60,17 +70,19 @@ __host__ __device__ constexpr uint32_t conv_tc_out_bytes() { return static_cast<
 template <int NT>
 __host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes() { return conv_tc_out_bytes<NT>() + static_cast<uint32_t>(NT) * kAccLd * 4; }
 
-// Row-strip mode (STRIP, 3x3 stride-1 dilation-1 convs with Cin % 64 == 0 on wide maps): a tile is 128 consecutive output
-// pixels of ONE row (tw = 128, th = 1).  Per 64-channel chunk the producer loads the 3 input rows x 130 pixels the tile needs
-// (left/right halo included) ONCE into a window buffer (ring of 2); the operand of tap (r,s) is the same window read through a
-// descriptor whose start address is shifted by r rows and s pixels (TMA and wgmma both apply the 128B swizzle to absolute
-// shared-memory address bits, so a 128B-multiple shift inside the 1024B-aligned window reads back what TMA wrote).  Only the
-// weights stream per (chunk, tap), through the stage ring.  The input is fetched 3x per chunk instead of 9x.
-constexpr uint32_t kWinBytes = 3 * (kTileM + 2) * 128;
-constexpr uint32_t kWinStride = (kWinBytes + 1023) / 1024 * 1024;
+// Window mode (WIN: 3x3 stride-1 dilation-1 convs without custom tap tables).  Per 64-channel chunk the producer loads the
+// (th + 2) x (tw + 2) input pixels the tile needs (halo included, out-of-image pixels and channels >= Cin zero-filled by TMA)
+// ONCE into a window buffer (ring of 2); the operand of tap (r,s) is the same window read through a descriptor whose start
+// address is shifted by r window rows and s pixels (TMA and wgmma both apply the 128B swizzle to absolute shared-memory
+// address bits, so a 128B-multiple shift inside the 1024B-aligned window reads back what TMA wrote).  Only the weights stream
+// per (chunk, tap), through the stage ring.  Every input byte of a tile crosses L2 -> SM about 1.4x per chunk instead of 9x.
+// Each m64 half of the 128-pixel tile must be 8 groups of 8 window-contiguous pixels at one stride:
+//   16 x 8 tiles: half h = the 8 x 8 block at columns 8h..8h+7, groups = tile rows (stride tw + 2 pixels);
+//   8 x 16 tiles: half h = tile rows 8h..8h+7, groups = tile rows (stride tw + 2 pixels);
+//   row strip (128 x 1 tiles, FSB_CONV_TC2=2): half h = pixels 64h..64h+63 of the row, groups 8 pixels apart.
 
-template <int BK, int NT, bool STRIP>
-__global__ void __launch_bounds__(kThreads, (NT <= 64 && !STRIP) ? 2 : 1)
+template <int BK, int NT, bool WIN>
+__global__ void __launch_bounds__(kThreads, NT <= 64 ? 2 : 1)
 conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
@@ -84,8 +96,8 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   constexpr uint32_t kABytes = kTileM * BK * 2;
-  constexpr uint32_t kStageBytes = STRIP ? NT * BK * 2 : kABytes + NT * BK * 2;
-  static_assert(!STRIP || BK == 64, "row-strip windows are 128B-swizzled 64-channel rows");
+  constexpr uint32_t kStageBytes = WIN ? NT * BK * 2 : kABytes + NT * BK * 2;
+  static_assert(!WIN || BK == 64, "windows are 128B-swizzled 64-channel rows");
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   // tile coordinates
@@ -122,15 +134,16 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   }
   __syncthreads();
 
-  if (STRIP && warp == 0) {
-    // ================= TMA producer, row strip: one input window per chunk, one weight tile per (chunk, tap) =================
-    uint8_t* bring = smem + 2 * kWinStride;
+  if (WIN && warp == 0) {
+    // ================= TMA producer, window mode: one input window per chunk, one weight tile per (chunk, tap) =================
+    uint8_t* bring = smem + 2 * p.win_stride;
+    const uint32_t win_bytes = static_cast<uint32_t>(p.win_rows * p.win_pitch) * 128u;
     RingPos rp, rw;
     for (int kc = 0; kc < p.k_chunks; ++kc) {
       mbar_wait_inline(&win_empty[rw.s], rw.phase ^ 1u);
       if (elect_one()) {
-        mbar_arrive_expect_tx(&win_full[rw.s], kWinBytes);
-        tma_load_4d(smem + rw.s * kWinStride, &p.tmap_a[0], &win_full[rw.s], kc * BK, w0 + p.tap_dw[0], h0 + p.tap_dh[0], img);
+        mbar_arrive_expect_tx(&win_full[rw.s], win_bytes);
+        tma_load_4d(smem + rw.s * p.win_stride, &p.tmap_a[0], &win_full[rw.s], kc * BK, w0 + p.tap_dw[0], h0 + p.tap_dh[0], img);
       }
       __syncwarp();
       rw.advance(2);
@@ -180,24 +193,25 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
     const uint64_t da0 = wgmma_desc_kmajor(sa0, BK * 2);
     const uint64_t db0 = wgmma_desc_kmajor(sa0 + kABytes, BK * 2);
     constexpr uint32_t kHalf = (64 * BK * 2) >> 4;  // pixel rows 64..127 of the A tile
-    if constexpr (STRIP) {
-      const uint64_t dw0 = wgmma_desc_kmajor(sa0, 128);                       // window 0, tap (0,0)
-      const uint64_t dbr = wgmma_desc_kmajor(sa0 + 2 * kWinStride, 128);      // weight ring, stage 0
+    if constexpr (WIN) {
+      const uint64_t dw0 = wgmma_desc(sa0, 16, p.win_sbo, 128);                // window 0, tap (0,0)
+      const uint64_t dbr = wgmma_desc_kmajor(sa0 + 2 * p.win_stride, 128);    // weight ring, stage 0
+      const uint64_t whalf = static_cast<uint64_t>(p.win_half * 8);           // win_half pixels x 128 B >> 4
       RingPos rp, rw;
       int prev = -1, prev_w = -1;
       for (int kc = 0; kc < p.k_chunks; ++kc) {
         mbar_wait_inline(&win_full[rw.s], rw.phase);
-        const uint64_t dwin = dw0 + static_cast<uint64_t>(rw.s * (kWinStride >> 4));
+        const uint64_t dwin = dw0 + static_cast<uint64_t>(rw.s * (p.win_stride >> 4));
         for (int tap = 0; tap < 9; ++tap) {
           const int r = tap / 3, sx = tap - 3 * r;
           mbar_wait_inline(&full_bar[rp.s], rp.phase);
           wgmma_fence();
-          const uint64_t da = dwin + static_cast<uint64_t>((r * (kTileM + 2) + sx) * 8);   // (r rows, sx pixels) x 128 B >> 4
+          const uint64_t da = dwin + static_cast<uint64_t>((r * p.win_pitch + sx) * 8);   // (r rows, sx pixels) x 128 B >> 4
           const uint64_t db = dbr + static_cast<uint64_t>(rp.s * (kStageBytes >> 4));
 #pragma unroll
           for (int k = 0; k < BK / 16; ++k) {
             wgmma_f16<NT, 0>(acc[0], da + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k));
-            wgmma_f16<NT, 0>(acc[1], da + kHalf + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k));
+            wgmma_f16<NT, 0>(acc[1], da + whalf + static_cast<uint64_t>(2 * k), db + static_cast<uint64_t>(2 * k));
           }
           wgmma_commit();
           wgmma_wait<1>();  // the previous group has read its operands
@@ -237,10 +251,22 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
     // has been consumed and every MMA has retired in all four warps once the barrier below is passed)
     float* s_acc = reinterpret_cast<float*>(smem + conv_tc_out_bytes<NT>());
     named_bar_sync(1, 128);
+    if constexpr (WIN) {
+      // this thread's fragment rows are row0 and row0 + 8 (8-row groups g0 and g0 + 1) of each half
+      const int row0 = wgmma_row(tw, 0);
+      const int m0 = (row0 >> 3) * p.m_grp + (row0 & 7);
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+      for (int h = 0; h < 2; ++h) {
+        float* s_h = s_acc + h * p.m_half + m0;
 #pragma unroll
-      for (int i = 0; i < NT / 2; ++i) s_acc[wgmma_col(tw, i) * kAccLd + 64 * h + wgmma_row(tw, i)] = acc[h][i];
+        for (int i = 0; i < NT / 2; ++i) s_h[wgmma_col(tw, i) * kAccLd + ((i >> 1) & 1) * p.m_grp] = acc[h][i];
+      }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < NT / 2; ++i) s_acc[wgmma_col(tw, i) * kAccLd + 64 * h + wgmma_row(tw, i)] = acc[h][i];
+    }
     named_bar_sync(1, 128);
 
     // ================= epilogue: thread m of the warpgroup owns pixel m of the tile =================
@@ -427,14 +453,21 @@ ConvGeom conv_geom(const fsb_conv_desc* d) {
   return g;
 }
 
-// Row-strip mode (see conv_tc_kernel): 3x3 stride-1 dilation-1 inference convs with 64-channel chunks, only with
-// FSB_CONV_TC2=2.  Off by default: on H100 it is slower than the per-tap mode on every 3x3 layer of the student frame (1.07-2x,
-// heads8 even) -- one CTA per SM (two 50 KB input windows) cannot hide its epilogue behind a second CTA, and the per-tap
-// mode's 9x input re-reads are served by L2 (tools/conv_bench.py --compare-strip, DESIGN.md section 3.3).
-bool conv_tc_strip(const fsb_conv_desc* d) {
-  if (d->ksize != 3 || d->stride != 1 || d->dil != 1 || d->Cin % 64 != 0 || (d->flags & FSB_CONV_STATS)) return false;
-  return opt(OPT_CONV_TC2) == 2;
+// Which conv_tc mode can run d (without custom tap tables).  3x3 stride-1 dilation-1 convs may use the window mode on their
+// 16 x 8 / 8 x 16 tiles: the per-tap mode moves every input byte of a tile from L2 to the SM nine times, and on large maps
+// L2 -> SM bandwidth, not HBM or the tensor cores, bounds the kernel (DESIGN.md section 3.3); conv_tc_launch takes it when the
+// grid has more CTAs than SMs.  FSB_CONV_TC2=0 forces the per-tap mode and 1 the window mode (for A/B measurements and tests);
+// FSB_CONV_TC2=2 selects the row strip (128 x 1 tiles, Cin % 64 == 0, no statistics), which is slower: its two 50 KB windows
+// allow one CTA per SM.
+enum ConvTcMode { kPerTap, kWindow, kStrip };
+static ConvTcMode conv_tc_mode(const fsb_conv_desc* d) {
+  if (d->ksize != 3 || d->stride != 1 || d->dil != 1) return kPerTap;
+  const int o = opt(OPT_CONV_TC2);
+  if (o == 0) return kPerTap;
+  if (o == 2 && d->Cin % 64 == 0 && !(d->flags & FSB_CONV_STATS)) return kStrip;
+  return kWindow;
 }
+bool conv_tc_strip(const fsb_conv_desc* d) { return conv_tc_mode(d) == kStrip; }
 
 // spatial tiles (= CTAs along M = partial statistic rows) of conv_tc
 int conv_tc_m_tiles(const fsb_conv_desc* d) {
@@ -449,28 +482,28 @@ int conv_tc_supported(const fsb_conv_desc* d) {
   return 1;
 }
 
-template <int BK, int NT, bool STRIP = false>
+template <int BK, int NT, bool WIN = false>
 static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcParams& p) {
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, STRIP>), 220 * 1024, "cudaFuncSetAttribute(conv_tc)"))
+  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, WIN>), 220 * 1024, "cudaFuncSetAttribute(conv_tc)"))
     return rc;
-  const cudaError_t e = launch_kernel(conv_tc_kernel<BK, NT, STRIP>, grid, dim3(kThreads), smem_bytes, stream, p);
+  const cudaError_t e = launch_kernel(conv_tc_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, p);
   return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
 }
 
-template <int BK, bool STRIP>
+template <int BK, bool WIN>
 static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcParams& p) {
   switch (n_tile) {
-    case 16: return conv_tc_run<BK, 16, STRIP>(grid, smem_bytes, stream, p);
-    case 32: return conv_tc_run<BK, 32, STRIP>(grid, smem_bytes, stream, p);
-    case 48: return conv_tc_run<BK, 48, STRIP>(grid, smem_bytes, stream, p);
-    case 64: return conv_tc_run<BK, 64, STRIP>(grid, smem_bytes, stream, p);
-    case 96: return conv_tc_run<BK, 96, STRIP>(grid, smem_bytes, stream, p);
-    default: return conv_tc_run<BK, 128, STRIP>(grid, smem_bytes, stream, p);
+    case 16: return conv_tc_run<BK, 16, WIN>(grid, smem_bytes, stream, p);
+    case 32: return conv_tc_run<BK, 32, WIN>(grid, smem_bytes, stream, p);
+    case 48: return conv_tc_run<BK, 48, WIN>(grid, smem_bytes, stream, p);
+    case 64: return conv_tc_run<BK, 64, WIN>(grid, smem_bytes, stream, p);
+    case 96: return conv_tc_run<BK, 96, WIN>(grid, smem_bytes, stream, p);
+    default: return conv_tc_run<BK, 128, WIN>(grid, smem_bytes, stream, p);
   }
 }
 
 int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu) {
+                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu, bool window_ok) {
   const ConvGeom g = conv_geom(d);
   if (cu && (d->stride != 1 || (d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS))))
     return set_error(FSB_ERR_INVALID, "conv_tc: custom tap tables need a stride-1 fp16 problem");
@@ -478,11 +511,11 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     return set_error(FSB_ERR_INVALID, "conv_tc: x / wpacked must be 16-byte aligned");
   ConvTcParams p;
   memset(&p, 0, sizeof(p));
+  const ConvTcMode mode = cu ? kPerTap : conv_tc_mode(d);
+  const bool strip = mode == kStrip;
   p.taps = cu ? cu->ntaps : g.taps;
-  p.k_chunks = g.kpad / g.bk;
   p.Ho = cu ? cu->Ho : d->Ho;
   p.Wo = cu ? cu->Wo : d->Wo;
-  const bool strip = !cu && conv_tc_strip(d);
   p.tw = strip ? kTileM : (p.Wo >= 16 ? 16 : 8);
   p.th = kTileM / p.tw;
   p.tiles_w = (p.Wo + p.tw - 1) / p.tw;
@@ -508,6 +541,35 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     n_tile = kNt[--ni];
     n_tiles = (g.npad + n_tile - 1) / n_tile;
   }
+  // A grid of at most one CTA per SM is bound by each CTA's latency, not by L2 -> SM traffic; there the window mode's wait for
+  // a whole window before the first MMA makes it slower (by 7-19 % on the student's 1/16 and 1/32 maps), so it runs only on
+  // larger grids unless FSB_CONV_TC2=1 forces it.  The training convs (BN-train statistics, and the data gradient, whose
+  // caller passes window_ok = false) stay per-tap: with them in window mode the distillation step measured slower.
+  const bool win = strip || (mode == kWindow && ((window_ok && m_tiles * n_tiles > sms && !(d->flags & FSB_CONV_STATS)) ||
+                                                 opt(OPT_CONV_TC2) == 1));
+  // window mode: 64-channel chunks for every Cin; a ragged last chunk is zero-filled by TMA on both operands (the input map
+  // ends at Cin, the weight map at kpad)
+  const int bk = win ? 64 : g.bk;
+  p.k_chunks = (g.kpad + bk - 1) / bk;
+  if (win) {
+    p.win_pitch = p.tw + 2;
+    p.win_rows = p.th + 2;
+    p.win_stride = (p.win_rows * p.win_pitch * 128 + 1023) / 1024 * 1024;
+    p.m_half = 64;
+    p.m_grp = 8;
+    if (strip) {
+      p.win_sbo = 8 * 128;
+      p.win_half = 64;
+    } else if (p.tw == 16) {
+      p.win_sbo = p.win_pitch * 128;
+      p.win_half = 8;
+      p.m_half = 8;
+      p.m_grp = 16;
+    } else {
+      p.win_sbo = p.win_pitch * 128;
+      p.win_half = 8 * p.win_pitch;
+    }
+  }
   p.y_cstride = d->y_cstride;
   p.flags = d->flags;
   p.scale = scale;
@@ -519,13 +581,14 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   if ((d->flags & FSB_CONV_STATS) && stats && (d->stats_off < 0 || d->stats_off + d->Cout > p.stats_C))
     return set_error(FSB_ERR_INVALID, "conv_tc: stats_off + Cout exceeds stats_C");
 
-  const size_t stage_bytes = (strip ? 0 : static_cast<size_t>(kTileM) * g.bk * 2) + static_cast<size_t>(n_tile) * g.bk * 2;
+  const size_t stage_bytes = (win ? 0 : static_cast<size_t>(kTileM) * bk * 2) + static_cast<size_t>(n_tile) * bk * 2;
   const int k_iters = p.taps * p.k_chunks;
   // 128-channel tiles hold 128 accumulator registers per thread: one CTA per SM, give the pipeline (almost) the whole shared
-  // memory; the same when the grid has at most one CTA per SM anyway.  Otherwise keep two CTAs per SM resident.
-  const size_t smem_budget = (n_tile == 128 || m_tiles * n_tiles <= sms) ? 200 * 1024 : 100 * 1024;
-  const size_t win_bytes = strip ? 2 * kWinStride : 0;   // row strip: two input windows ahead of the weight ring
-  int stages = static_cast<int>((strip ? 200 * 1024 - win_bytes : smem_budget) / stage_bytes);
+  // memory; the same when the grid has at most one CTA per SM anyway (and for the row strip, whose windows alone take 100 KB).
+  // Otherwise keep two CTAs per SM resident.
+  const size_t smem_budget = (n_tile == 128 || m_tiles * n_tiles <= sms || strip) ? 200 * 1024 : 100 * 1024;
+  const size_t win_bytes = win ? 2 * static_cast<size_t>(p.win_stride) : 0;   // two input windows ahead of the weight ring
+  int stages = static_cast<int>((smem_budget - win_bytes) / stage_bytes);
   if (stages < 2) stages = 2;
   if (stages > kMaxStages) stages = kMaxStages;
   if (stages > k_iters) stages = k_iters;
@@ -564,13 +627,13 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   // ---- A tensor maps ----
   const __half* xb = static_cast<const __half*>(x);
   const uint64_t cs = static_cast<uint64_t>(d->x_cstride) * 2;  // bytes per pixel step
-  const uint32_t boxA[4] = {static_cast<uint32_t>(g.bk), static_cast<uint32_t>(strip ? kTileM + 2 : p.tw),
-                            static_cast<uint32_t>(strip ? 3 : p.th), 1u};
+  const uint32_t boxA[4] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(win ? p.win_pitch : p.tw),
+                            static_cast<uint32_t>(win ? p.win_rows : p.th), 1u};
   if (d->stride == 1) {
     const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
                               static_cast<uint64_t>(d->N)};
     const uint64_t str[3] = {cs, cs * d->W, cs * d->W * d->H};
-    int rc = encode_tiled(&p.tmap_a[0], xb, 4, dims, str, boxA, g.bk * 2);
+    int rc = encode_tiled(&p.tmap_a[0], xb, 4, dims, str, boxA, bk * 2);
     if (rc) return rc;
     for (int r = 0; r < d->ksize; ++r)
       for (int s = 0; s < d->ksize; ++s) {
@@ -618,12 +681,12 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   {
     const uint64_t dims[3] = {static_cast<uint64_t>(g.kpad), static_cast<uint64_t>(g.npad), static_cast<uint64_t>(g.taps)};
     const uint64_t str[2] = {static_cast<uint64_t>(g.kpad) * 2, static_cast<uint64_t>(g.kpad) * g.npad * 2};
-    const uint32_t boxB[3] = {static_cast<uint32_t>(g.bk), static_cast<uint32_t>(n_tile), 1u};
-    int rc = encode_tiled(&p.tmap_b, wpacked, 3, dims, str, boxB, g.bk * 2);
+    const uint32_t boxB[3] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(n_tile), 1u};
+    int rc = encode_tiled(&p.tmap_b, wpacked, 3, dims, str, boxB, bk * 2);
     if (rc) return rc;
   }
   const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles));
-  if (strip) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, p);
+  if (win) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, p);
   if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, p);
   return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, p);
 }

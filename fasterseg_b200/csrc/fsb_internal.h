@@ -35,7 +35,8 @@ int sm_count();
 // getenv() on the launch path.  -1 = unset.  The switches marked "no effect" selected conv kernel variants that this sm_90a
 // library does not have; their names stay accepted so that existing settings keep working.
 enum Opt {
-  OPT_CONV_TC2 = 0,      // FSB_CONV_TC2: 2 = row-strip mode of conv_tc wherever the geometry allows (default: per-tap)
+  OPT_CONV_TC2 = 0,      // FSB_CONV_TC2: mode of conv_tc for 3x3 stride-1 convs: 0 = per-tap, 1 = window, 2 = row strip
+                         // (default: window on inference convs with more CTAs than SMs, else per-tap)
   OPT_TC2_R,             // FSB_TC2_R: no effect
   OPT_TC2_ASTAGES,       // FSB_TC2_ASTAGES: no effect
   OPT_NO_TMA_STORE,      // FSB_NO_TMA_STORE
@@ -100,8 +101,9 @@ struct ConvTcCustom {
 };
 int conv_tc_supported(const fsb_conv_desc* d);
 bool conv_tc_strip(const fsb_conv_desc* d);  // conv_tc runs d in row-strip mode
+// window_ok = false keeps a 3x3 stride-1 problem on the per-tap mode unless FSB_CONV_TC2 forces the window mode
 int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr);
+                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr, bool window_ok = true);
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride);
 int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
                          float gscale, cudaStream_t stream);

@@ -378,7 +378,7 @@ int conv_dgrad_launch(const fsb_conv_desc* d, const void* dy, int dcs, const voi
                       int64_t si, void* dx, int xcs, cudaStream_t stream) {
   if (d->stride == 1 && d->off_h == 0 && d->off_w == 0 && wpacked_t && !(d->flags & FSB_CONV_FORCE_DIRECT)) {
     fsb_conv_desc t = dgrad_as_fwd_desc(d, dcs, xcs);
-    if (conv_tc_supported(&t)) return conv_tc_launch(&t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream);
+    if (conv_tc_supported(&t)) return conv_tc_launch(&t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream, nullptr, false);
   }
   // stride 2: the input pixels of each (row, column) parity receive contributions from a fixed subset of filter taps; each
   // parity plane is a stride-1 implicit GEMM over dy with that tap subset, written to the plane through a strided tensor map

@@ -133,8 +133,9 @@ int fsb_bn_fold(int C, const float* gamma, const float* beta, const float* mean,
  * NHWC tiles; Cin < 16 (the RGB stem) and FSB_CONV_FORCE_DIRECT use the CUDA-core direct kernel. */
 int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
                  void* y, float* stats, void* stream);
-/* which kernel fsb_conv_fwd dispatches for `d`: 0 = CUDA-core direct, 1 = per-tap wgmma (conv_tc), 2 = conv_tc in row-strip
- * mode (one input window per channel chunk, taps as descriptor offsets); negative = invalid descriptor.  y and with_stats are
+/* which kernel fsb_conv_fwd dispatches for `d`: 0 = CUDA-core direct, 1 = the wgmma kernel conv_tc on 16x8 / 8x16 pixel tiles
+ * (per-tap mode, or window mode: one halo window of the input per 64-channel chunk, taps as descriptor offsets), 2 = conv_tc
+ * in row-strip mode (the window mode on 128x1 tiles, FSB_CONV_TC2=2); negative = invalid descriptor.  y and with_stats are
  * accepted for compatibility and do not change the choice. */
 int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats);
 /* number of partial statistic rows fsb_conv_fwd writes for `d` with FSB_CONV_STATS (depends on the kernel it dispatches):

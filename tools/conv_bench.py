@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """Per-layer micro-benchmark of the conv / resize kernels on the student's layer shapes (1x3x1024x2048 frame).
 Prints us/launch, achieved TFLOP/s and algorithmic GB/s per layer; `--only i` restricts to one layer.
-`--compare-strip`: on every layer the row-strip mode of conv_tc can run, time it (FSB_CONV_TC2=2) against the per-tap mode
-(FSB_CONV_TC2=0), alternating the two `--rounds` times in this process, and print the median of each."""
+`--compare`: on every layer time conv_tc's per-tap mode (FSB_CONV_TC2=0), its default (window mode on 3x3 stride-1 convs) and,
+where it applies, the row strip (FSB_CONV_TC2=2), alternating them `--rounds` times in this process; print the median us of
+each and the L2 -> SM bytes each mode moves (TMA boxes of input and weights, from conv_tc_launch's tiling rule)."""
 import argparse
 import os
 import sys
@@ -44,12 +45,43 @@ LAYERS = [
 ]
 
 
+SMS = 132  # H100 SXM
+
+
+def l2_to_sm_mb(ci, co, k, s, h, w, mode):
+    """(MB of TMA boxes one launch loads into shared memory in `mode` ("per-tap", "window" or "strip"), CTAs), following
+    conv_tc_launch: 16 x 8 tiles (8 x 16 when Wo < 16, 128 x 1 for the strip), N tile of <= 128 channels split while the grid has
+    fewer CTAs than SMs; per-tap: one input box of 128 px x BK and one weight box per (tap, chunk); window / strip: one
+    (th + 2) x (tw + 2) px x 64-channel window per chunk and one weight box per (chunk, tap)."""
+    pad = 1 if k == 3 else 0
+    ho, wo = (h + 2 * pad - k) // s + 1, (w + 2 * pad - k) // s + 1
+    tw = 128 if mode == "strip" else (16 if wo >= 16 else 8)
+    th = 128 // tw
+    m_tiles = -(-wo // tw) * -(-ho // th)
+    npad = -(-co // 16) * 16
+    nts = [16, 32, 48, 64, 96, 128]
+    n_tiles = -(-npad // 128)
+    ni = next(i for i, nt in enumerate(nts) if nt * n_tiles >= npad)
+    n_tiles = -(-npad // nts[ni])
+    while m_tiles * n_tiles < SMS and ni > 0 and nts[ni - 1] >= 32:
+        ni -= 1
+        n_tiles = -(-npad // nts[ni])
+    nt = nts[ni]
+    bk = 64 if (mode != "per-tap" or ci % 64 == 0) else 32
+    chunks = -(-ci // bk)
+    if mode == "per-tap":
+        per_cta = k * k * chunks * (128 + nt) * bk * 2
+    else:
+        per_cta = chunks * ((th + 2) * (tw + 2) * 128 + 9 * nt * 128)
+    return m_tiles * n_tiles * per_cta / 1e6, m_tiles * n_tiles
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--only", type=int, default=-1)
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--direct", action="store_true")
-    ap.add_argument("--compare-strip", action="store_true")
+    ap.add_argument("--compare", action="store_true")
     ap.add_argument("--rounds", type=int, default=5)
     args = ap.parse_args()
     dev = torch.device("cuda")
@@ -91,20 +123,27 @@ def main():
             en.synchronize()
             return st.elapsed_time(en) * 1000 / args.reps
 
-        if args.compare_strip:
-            if not (k == 3 and s == 1 and ci % 64 == 0):
-                continue
+        if args.compare:
+            # FSB_CONV_TC2: 0 = per-tap, 1 = window, 2 = row strip; unset (the default) = window on grids of more CTAs than SMs
+            modes = {"per-tap": 0, "window": 1, "strip": 2} if k == 3 and s == 1 else {"per-tap": 0}
+            if ci % 64 != 0:
+                modes.pop("strip", None)
             graphs = {}
-            for mode in (0, 2):
-                _lib.set_option("FSB_CONV_TC2", mode)
-                graphs[mode] = timed_graph()
+            for label, v in modes.items():
+                _lib.set_option("FSB_CONV_TC2", v)
+                graphs[label] = timed_graph()
             _lib.set_option("FSB_CONV_TC2", -1)
-            ts = {0: [], 2: []}
+            ts = {label: [] for label in modes}
             for _ in range(args.rounds):
-                for mode in (0, 2):
-                    ts[mode].append(replay_us(graphs[mode]))
-            t0, t2 = sorted(ts[0])[len(ts[0]) // 2], sorted(ts[2])[len(ts[2]) // 2]
-            print("%2d %-18s %3d->%3d %4dx%-4d  per-tap %8.2f us  row-strip %8.2f us  ratio %.3f" % (li, name, ci, co, h, w, t0, t2, t2 / t0))
+                for label in modes:
+                    ts[label].append(replay_us(graphs[label]))
+            med = {label: sorted(v)[len(v) // 2] for label, v in ts.items()}
+            cols = "  ".join("%s %8.2f us %6.1f MB" % (label, med[label], l2_to_sm_mb(ci, co, k, s, h, w, label)[0])
+                             for label in modes)
+            ctas = l2_to_sm_mb(ci, co, k, s, h, w, "per-tap")[1]
+            default = "window" if "window" in modes and ctas > SMS else "per-tap"
+            print("%2d %-18s %3d->%3d k%d s%d %4dx%-4d %4d CTAs  %s  per-tap/window %.2fx  default %s" % (
+                li, name, ci, co, k, s, h, w, ctas, cols, med["per-tap"] / med.get("window", med["per-tap"]), default))
             continue
         us = replay_us(timed_graph())
         flops = 2.0 * k * k * ci * co * ho * wo
