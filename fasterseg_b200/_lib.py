@@ -14,6 +14,8 @@ FSB_CONV_FORCE_DIRECT = 4
 FSB_CONV_STATS = 8
 FSB_CONV_OUT_F32 = 16
 FSB_ACT_IN_F32 = 32
+FSB_CONV_X_DOWN2 = 64
+FSB_CONV_Y_UP2 = 128
 ABI_VERSION = 2
 
 
@@ -58,6 +60,9 @@ _SIGS = {
     "fsb_bilinear_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, C.c_uint32, _P]),
     "fsb_upsample_logits_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_argmax": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),
+    "fsb_nearest_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
+    "fsb_upsample_logits_nearest_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
+    "fsb_upsample_argmax_nearest": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),
     "fsb_nchw_to_nhwc_f16": (C.c_int, [C.c_int] * 4 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_nhwc_f16_to_nchw": (C.c_int, [C.c_int] * 4 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_copy_channels": (C.c_int, [C.c_int64, C.c_int, _P, C.c_int, _P, C.c_int, _P]),

@@ -56,7 +56,7 @@ int opt(Opt o) {
 
 int ensure_dyn_smem(const void* kernel, int bytes, const char* what) {
   struct Entry { const void* k; unsigned long long mask; };
-  static Entry table[32];
+  static Entry table[64];
   static int n = 0;
   static std::mutex mu;
   int dev = 0;
@@ -70,7 +70,7 @@ int ensure_dyn_smem(const void* kernel, int bytes, const char* what) {
   if (hit && (hit->mask & bit)) return FSB_OK;
   e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   if (e != cudaSuccess) return set_cuda_error(e, what);
-  if (!hit && n < 32) {
+  if (!hit && n < 64) {
     table[n].k = kernel;
     table[n].mask = 0;
     hit = &table[n++];
@@ -102,6 +102,9 @@ int confusion_launch(int64_t, const uint8_t*, const void*, int, int, long long*,
 int bilinear_launch(int, int, int, int, int, int, const void*, int, void*, int, uint32_t, cudaStream_t);
 int upsample_logits_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
+int nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
+int upsample_logits_nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
+int upsample_argmax_nearest_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
 int nchw_to_nhwc_launch(int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int nhwc_to_nchw_launch(int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int copy_channels_launch(int64_t, int, const void*, int, void*, int, cudaStream_t);
@@ -291,7 +294,11 @@ int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, con
   if (rc) return rc;
   if (!x || !wpacked || !y) return set_error(FSB_ERR_INVALID, "conv_fwd: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d)) return conv_direct_launch(d, x, wpacked, scale, shift, y, stats, st);
+  const bool direct = (d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d);
+  if (direct && (d->flags & (FSB_CONV_X_DOWN2 | FSB_CONV_Y_UP2)))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd: FSB_CONV_X_DOWN2 / FSB_CONV_Y_UP2 need the wgmma kernel (Cin >= 16, x_cstride % 8 == 0, "
+                                          "no FSB_CONV_FORCE_DIRECT)");
+  if (direct) return conv_direct_launch(d, x, wpacked, scale, shift, y, stats, st);
   return conv_tc_launch(d, x, wpacked, scale, shift, y, stats, st);
 }
 
@@ -328,6 +335,23 @@ int fsb_upsample_logits_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const
 int fsb_upsample_argmax(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, uint8_t* labels, void* stream) {
   if (N <= 0 || C <= 0 || C > 255 || !x || !labels || xcs < C) return set_error(FSB_ERR_INVALID, "upsample_argmax: bad argument");
   return upsample_argmax_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, labels, static_cast<cudaStream_t>(stream));
+}
+
+int fsb_nearest_fwd(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int ycs, void* stream) {
+  if (N <= 0 || C <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !y || xcs < C || ycs < C)
+    return set_error(FSB_ERR_INVALID, "nearest: bad argument");
+  return nearest_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, y, ycs, static_cast<cudaStream_t>(stream));
+}
+int fsb_upsample_logits_nearest_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int out_dtype,
+                                     void* stream) {
+  if (N <= 0 || C <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !y || xcs < C || (out_dtype != 0 && out_dtype != 1))
+    return set_error(FSB_ERR_INVALID, "upsample_logits_nearest: bad argument");
+  return upsample_logits_nearest_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, y, out_dtype, static_cast<cudaStream_t>(stream));
+}
+int fsb_upsample_argmax_nearest(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, uint8_t* labels, void* stream) {
+  if (N <= 0 || C <= 0 || C > 255 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !labels || xcs < C)
+    return set_error(FSB_ERR_INVALID, "upsample_argmax_nearest: bad argument");
+  return upsample_argmax_nearest_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, labels, static_cast<cudaStream_t>(stream));
 }
 
 int fsb_nchw_to_nhwc_f16(int N, int C, int H, int W, const void* x, int x_is_f32, void* y, int ycs, void* stream) {

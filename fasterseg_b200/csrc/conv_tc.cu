@@ -63,6 +63,15 @@ struct ConvTcParams {
   int stats_off;  // channel offset of this conv's output inside a row
 };
 
+// Parameters of the FSB_CONV_Y_UP2 instances: the staged output goes to y_reps = 4 lattices (one per 2x2 parity), lattice 0
+// through p.tmap_y, lattice l >= 1 through tmap_up[2l - 2] (64-channel slabs) and tmap_up[2l - 1] (tail slab).  A struct of its
+// own, so that every other launch keeps ConvTcParams' size (kernel-parameter bytes are uploaded per launch).
+struct ConvTcUp2Params {
+  ConvTcParams p;
+  int y_reps;
+  CUtensorMap tmap_up[6];
+};
+
 // shared memory after the main loop: [0, kOutBytes) = statistics partials or the TMA-store staging slabs,
 // [kOutBytes, + NT * kAccLd * 4) = the parked accumulator; both reuse the (then idle) stage ring
 template <int NT>
@@ -81,9 +90,10 @@ __host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes() { return conv_tc
 //   8 x 16 tiles: half h = tile rows 8h..8h+7, groups = tile rows (stride tw + 2 pixels);
 //   row strip (128 x 1 tiles, FSB_CONV_TC2=2): half h = pixels 64h..64h+63 of the row, groups 8 pixels apart.
 
-template <int BK, int NT, bool WIN>
-__global__ void __launch_bounds__(kThreads, NT <= 64 ? 2 : 1)
-conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
+// The kernel body.  UP2 (FSB_CONV_Y_UP2) only adds the stores of each staged slab to lattices 1 .. y_reps - 1; it is compiled
+// into instances of its own (conv_tc_up2_kernel) so that the instances every other call runs keep their registers.
+template <int BK, int NT, bool WIN, bool UP2>
+__device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtensorMap* tmap_up, int y_reps) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
@@ -377,6 +387,10 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
         if (warp == 4 && lane == 0) {
           const bool full = (NT - c0) >= 64;
           tma_store_4d(&p.tmap_y[full ? 0 : 1], smem + static_cast<size_t>(c0 >> 6) * (kTileM * 128), n0 + c0, w0, h0, img);
+          if constexpr (UP2)
+            for (int l = 1; l < y_reps; ++l)
+              tma_store_4d(&tmap_up[2 * l - 2 + (full ? 0 : 1)], smem + static_cast<size_t>(c0 >> 6) * (kTileM * 128), n0 + c0, w0,
+                           h0, img);
           tma_store_commit();
         }
       }
@@ -401,6 +415,18 @@ conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
     }
   }
   __syncthreads();
+}
+
+template <int BK, int NT, bool WIN>
+__global__ void __launch_bounds__(kThreads, NT <= 64 ? 2 : 1)
+conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
+  conv_tc_body<BK, NT, WIN, false>(p, nullptr, 1);
+}
+
+template <int BK, int NT, bool WIN>
+__global__ void __launch_bounds__(kThreads, NT <= 64 ? 2 : 1)
+conv_tc_up2_kernel(const __grid_constant__ ConvTcUp2Params q) {
+  conv_tc_body<BK, NT, WIN, true>(q.p, q.tmap_up, q.y_reps);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -483,22 +509,25 @@ int conv_tc_supported(const fsb_conv_desc* d) {
 }
 
 template <int BK, int NT, bool WIN = false>
-static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcParams& p) {
-  if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, WIN>), 220 * 1024, "cudaFuncSetAttribute(conv_tc)"))
-    return rc;
-  const cudaError_t e = launch_kernel(conv_tc_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, p);
+static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q) {
+  const bool up2 = q.y_reps > 1;
+  const void* kernel = up2 ? reinterpret_cast<const void*>(conv_tc_up2_kernel<BK, NT, WIN>)
+                           : reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, WIN>);
+  if (int rc = ensure_dyn_smem(kernel, 220 * 1024, "cudaFuncSetAttribute(conv_tc)")) return rc;
+  const cudaError_t e = up2 ? launch_kernel(conv_tc_up2_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, q)
+                            : launch_kernel(conv_tc_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, q.p);
   return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
 }
 
 template <int BK, bool WIN>
-static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcParams& p) {
+static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q) {
   switch (n_tile) {
-    case 16: return conv_tc_run<BK, 16, WIN>(grid, smem_bytes, stream, p);
-    case 32: return conv_tc_run<BK, 32, WIN>(grid, smem_bytes, stream, p);
-    case 48: return conv_tc_run<BK, 48, WIN>(grid, smem_bytes, stream, p);
-    case 64: return conv_tc_run<BK, 64, WIN>(grid, smem_bytes, stream, p);
-    case 96: return conv_tc_run<BK, 96, WIN>(grid, smem_bytes, stream, p);
-    default: return conv_tc_run<BK, 128, WIN>(grid, smem_bytes, stream, p);
+    case 16: return conv_tc_run<BK, 16, WIN>(grid, smem_bytes, stream, q);
+    case 32: return conv_tc_run<BK, 32, WIN>(grid, smem_bytes, stream, q);
+    case 48: return conv_tc_run<BK, 48, WIN>(grid, smem_bytes, stream, q);
+    case 64: return conv_tc_run<BK, 64, WIN>(grid, smem_bytes, stream, q);
+    case 96: return conv_tc_run<BK, 96, WIN>(grid, smem_bytes, stream, q);
+    default: return conv_tc_run<BK, 128, WIN>(grid, smem_bytes, stream, q);
   }
 }
 
@@ -507,10 +536,17 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   const ConvGeom g = conv_geom(d);
   if (cu && (d->stride != 1 || (d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS))))
     return set_error(FSB_ERR_INVALID, "conv_tc: custom tap tables need a stride-1 fp16 problem");
+  if (cu && (d->flags & (FSB_CONV_X_DOWN2 | FSB_CONV_Y_UP2)))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_X_DOWN2 / FSB_CONV_Y_UP2 cannot be combined with a custom output lattice");
+  if ((d->flags & FSB_CONV_X_DOWN2) && d->stride != 1)
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_X_DOWN2 needs a stride-1 conv");
+  if ((d->flags & FSB_CONV_Y_UP2) && (d->flags & (FSB_CONV_STATS | FSB_CONV_OUT_F32)))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_Y_UP2 cannot be combined with FSB_CONV_STATS or FSB_CONV_OUT_F32");
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(wpacked) & 15))
     return set_error(FSB_ERR_INVALID, "conv_tc: x / wpacked must be 16-byte aligned");
-  ConvTcParams p;
-  memset(&p, 0, sizeof(p));
+  ConvTcUp2Params q;
+  memset(&q, 0, sizeof(q));
+  ConvTcParams& p = q.p;
   const ConvTcMode mode = cu ? kPerTap : conv_tc_mode(d);
   const bool strip = mode == kStrip;
   p.taps = cu ? cu->ntaps : g.taps;
@@ -598,31 +634,49 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
                            : n_tile == 96 ? conv_tc_epilogue_bytes<96>() : conv_tc_epilogue_bytes<128>();
   size_t smem_bytes = (win_bytes + stage_bytes * stages > epi_bytes ? win_bytes + stage_bytes * stages : epi_bytes) + 1024;
   // ---- TMA-store epilogue: fp16 output whose pixels start on 16 B and whose channel count is a multiple of 8 ----
+  // FSB_CONV_Y_UP2: y is the 2Ho x 2Wo map and every output pixel goes to its 2x2 block (nearest x2 folded into the store):
+  // four lattice maps, one per (row, column) parity, each with the pixel steps of the full map doubled; the epilogue stores
+  // every staged slab to each of them.
+  const bool up2 = (d->flags & FSB_CONV_Y_UP2) != 0;
   p.tma_store = 0;
+  q.y_reps = 1;
   if (!(d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS)) && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
-      n_tile % 8 == 0 && (cu || opt(OPT_NO_TMA_STORE) <= 0)) {
+      n_tile % 8 == 0 && (cu || up2 || opt(OPT_NO_TMA_STORE) <= 0)) {
     const uint64_t ycs = static_cast<uint64_t>(d->y_cstride) * 2;
     uint64_t dims[4] = {static_cast<uint64_t>(d->Cout), static_cast<uint64_t>(d->Wo), static_cast<uint64_t>(d->Ho),
                         static_cast<uint64_t>(d->N)};
     uint64_t str[3] = {ycs, ycs * d->Wo, ycs * d->Wo * d->Ho};
+    const uint8_t* ybase[4] = {static_cast<const uint8_t*>(y), nullptr, nullptr, nullptr};
     if (cu) {  // output = a strided sub-lattice (parity plane) of the destination tensor
-      y = const_cast<void*>(cu->y_base);
+      ybase[0] = static_cast<const uint8_t*>(cu->y_base);
       for (int i = 0; i < 4; ++i) dims[i] = cu->y_dims[i];
       for (int i = 0; i < 3; ++i) str[i] = cu->y_strides[i];
     }
-    const uint32_t box64[4] = {64u, static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
-    int rc = 0;
-    if (n_tile >= 64) rc = encode_tiled(&p.tmap_y[0], y, 4, dims, str, box64, 128);
-    p.tail_w = n_tile % 64;
-    if (!rc && p.tail_w) {
-      const uint32_t boxt[4] = {static_cast<uint32_t>(p.tail_w), static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
-      rc = encode_tiled(&p.tmap_y[1], y, 4, dims, str, boxt, 0);
+    if (up2) {
+      q.y_reps = 4;
+      const uint64_t row = ycs * 2 * d->Wo;  // one row of the 2Ho x 2Wo map
+      str[0] = 2 * ycs;
+      str[1] = 2 * row;
+      str[2] = row * 2 * d->Ho;
+      for (int l = 0; l < 4; ++l) ybase[l] = static_cast<const uint8_t*>(y) + (l >> 1) * row + (l & 1) * ycs;
     }
-    if (rc) return rc;
-    if (n_tile < 64) p.tmap_y[0] = p.tmap_y[1];
+    const uint32_t box64[4] = {64u, static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
+    p.tail_w = n_tile % 64;
+    const uint32_t boxt[4] = {static_cast<uint32_t>(p.tail_w), static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
+    for (int l = 0; l < q.y_reps; ++l) {
+      CUtensorMap* maps = l == 0 ? p.tmap_y : q.tmap_up + 2 * (l - 1);
+      int rc = 0;
+      if (n_tile >= 64) rc = encode_tiled(&maps[0], ybase[l], 4, dims, str, box64, 128);
+      if (!rc && p.tail_w) rc = encode_tiled(&maps[1], ybase[l], 4, dims, str, boxt, 0);
+      if (rc) return rc;
+      if (n_tile < 64) maps[0] = maps[1];
+    }
     p.tma_store = 1;
   }
   if (cu && !p.tma_store) return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: custom output lattice needs the TMA-store epilogue");
+  if (up2 && !p.tma_store)
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_Y_UP2 needs the TMA-store epilogue (fp16 output, Cout and y_cstride "
+                                          "multiples of 8, 16-byte aligned y)");
 
   // ---- A tensor maps ----
   const __half* xb = static_cast<const __half*>(x);
@@ -632,7 +686,9 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   if (d->stride == 1) {
     const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
                               static_cast<uint64_t>(d->N)};
-    const uint64_t str[3] = {cs, cs * d->W, cs * d->W * d->H};
+    // FSB_CONV_X_DOWN2: x is the 2H x 2W map and the conv reads its even rows and columns (nearest /2 folded into the load)
+    const bool down2 = (d->flags & FSB_CONV_X_DOWN2) != 0;
+    const uint64_t str[3] = {down2 ? 2 * cs : cs, down2 ? 4 * cs * d->W : cs * d->W, down2 ? 4 * cs * d->W * d->H : cs * d->W * d->H};
     int rc = encode_tiled(&p.tmap_a[0], xb, 4, dims, str, boxA, bk * 2);
     if (rc) return rc;
     for (int r = 0; r < d->ksize; ++r)
@@ -686,9 +742,9 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     if (rc) return rc;
   }
   const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles));
-  if (win) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, p);
-  if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, p);
-  return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, p);
+  if (win) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, q);
+  if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, q);
+  return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, q);
 }
 
 }  // namespace fsb

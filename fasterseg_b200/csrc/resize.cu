@@ -493,6 +493,193 @@ int upsample_argmax_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const v
 }
 
 // ------------------------------------------------------------------------------------------
+// nearest (latency/ deployment network): torch's legacy 'nearest' index rule, scale and product in fp32 -- for sizes like
+// 5 -> 2 or 2 -> 5 the float rounding IS the behaviour, so no integer shortcut.  Pure copies: outputs are bit-exact.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ int nearest_src(int dst, int n_in, int n_out) {
+  const float scale = static_cast<float>(n_in) / static_cast<float>(n_out);
+  const int s = static_cast<int>(floorf(static_cast<float>(dst) * scale));
+  return s < n_in - 1 ? s : n_in - 1;
+}
+
+// one thread = one output pixel x 8 channels
+__global__ void __launch_bounds__(256)
+nearest_nhwc_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs, __half* __restrict__ y,
+                    int ycs) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int cvec = C >> 3;
+  const int64_t total = static_cast<int64_t>(N) * Ho * Wo * cvec;
+  const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (gid >= total) return;
+  const int cv = static_cast<int>(gid % cvec);
+  const int64_t pix = gid / cvec;
+  const int wo = static_cast<int>(pix % Wo);
+  const int ho = static_cast<int>((pix / Wo) % Ho);
+  const int n = static_cast<int>(pix / (static_cast<int64_t>(Wo) * Ho));
+  const int hs = nearest_src(ho, Hi, Ho), ws = nearest_src(wo, Wi, Wo);
+  *reinterpret_cast<uint4*>(y + static_cast<size_t>(pix) * ycs + cv * 8) =
+      *reinterpret_cast<const uint4*>(x + ((static_cast<size_t>(n) * Hi + hs) * Wi + ws) * xcs + cv * 8);
+}
+
+int nearest_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int ycs, cudaStream_t stream) {
+  if (C % 8 || xcs % 8 || ycs % 8 || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15))
+    return set_error(FSB_ERR_INVALID, "nearest: C, strides must be multiples of 8 and pointers 16B aligned");
+  const int64_t total = static_cast<int64_t>(N) * Ho * Wo * (C / 8);
+  FSB_LAUNCH(nearest_nhwc_kernel, dim3(static_cast<unsigned>((total + 255) / 256)), dim3(256), 0, stream, N, C, Hi, Wi, Ho, Wo,
+             static_cast<const __half*>(x), xcs, static_cast<__half*>(y), ycs);
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "nearest launch");
+  return FSB_OK;
+}
+
+// final nearest logits upsample: NHWC fp16 -> NCHW.  One thread = 8 consecutive output columns of one output row, all classes;
+// per class it stores one 16-byte vector (fp16) or two (fp32), so a warp writes 512 / 1024 contiguous bytes.  The kernel is
+// bound by these writes; the source values (one or two pixels per thread at x8) come from L1.
+template <typename TOut>
+__global__ void __launch_bounds__(128)
+upsample_logits_nearest_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs,
+                               TOut* __restrict__ y) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int wvec = (Wo + 7) >> 3;
+  const int64_t total = static_cast<int64_t>(N) * Ho * wvec;
+  const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (gid >= total) return;
+  const int wv = static_cast<int>(gid % wvec);
+  const int ho = static_cast<int>((gid / wvec) % Ho);
+  const int n = static_cast<int>(gid / (static_cast<int64_t>(wvec) * Ho));
+  const __half* row = x + (static_cast<size_t>(n) * Hi + nearest_src(ho, Hi, Ho)) * Wi * xcs;
+  int ws[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) ws[j] = nearest_src(min(wv * 8 + j, Wo - 1), Wi, Wo);
+  const size_t plane = static_cast<size_t>(Ho) * Wo;
+  TOut* yrow = y + static_cast<size_t>(n) * C * plane + static_cast<size_t>(ho) * Wo + wv * 8;
+  const bool full = (wv * 8 + 8 <= Wo) && ((reinterpret_cast<uintptr_t>(yrow) & 15) == 0) && ((plane * sizeof(TOut)) % 16 == 0);
+  for (int c = 0; c < C; ++c) {
+    float o[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+      o[j] = (j > 0 && ws[j] == ws[j - 1]) ? o[j - 1] : __half2float(row[static_cast<size_t>(ws[j]) * xcs + c]);
+    TOut* dst = yrow + static_cast<size_t>(c) * plane;
+    if (full) {
+      if (sizeof(TOut) == 2) {
+        uint4 v;
+        v.x = pack_half2(o[0], o[1]);
+        v.y = pack_half2(o[2], o[3]);
+        v.z = pack_half2(o[4], o[5]);
+        v.w = pack_half2(o[6], o[7]);
+        *reinterpret_cast<uint4*>(dst) = v;
+      } else {
+        float4* d4 = reinterpret_cast<float4*>(dst);
+        d4[0] = make_float4(o[0], o[1], o[2], o[3]);
+        d4[1] = make_float4(o[4], o[5], o[6], o[7]);
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        if (wv * 8 + j < Wo) dst[j] = static_cast<TOut>(o[j]);
+    }
+  }
+}
+
+int upsample_logits_nearest_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int out_dtype,
+                                   cudaStream_t stream) {
+  const int64_t total = static_cast<int64_t>(N) * Ho * ((Wo + 7) / 8);
+  const dim3 grid(static_cast<unsigned>((total + 127) / 128));
+  if (out_dtype == 0)
+    FSB_LAUNCH(upsample_logits_nearest_kernel<__half>, grid, dim3(128), 0, stream, N, C, Hi, Wi, Ho, Wo, static_cast<const __half*>(x),
+               xcs, static_cast<__half*>(y));
+  else
+    FSB_LAUNCH(upsample_logits_nearest_kernel<float>, grid, dim3(128), 0, stream, N, C, Hi, Wi, Ho, Wo, static_cast<const __half*>(x),
+               xcs, static_cast<float*>(y));
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "upsample_logits_nearest launch");
+  return FSB_OK;
+}
+
+// nearest upsample + argmax -> uint8 labels.  A block owns kLabRows x kLabCols output pixels.  The nearest index is monotone,
+// so the source rows (columns) the tile touches are a run src0..src_last when upsampling (in <= out: consecutive outputs
+// differ by 0 or 1) and one distinct source per output when downsampling (in > out: they differ by >= 1).  The block takes
+// the argmax once per distinct source pixel into shared memory, then every thread stores 8 replicated labels (one 8-byte store).
+// Arithmetic: strict '>' over the fp16 values widened to fp32, i.e. the argmax of the logits kernel's output (which holds the
+// same values), first maximum winning.
+constexpr int kLabRows = 8;
+constexpr int kLabCols = 256;
+
+__global__ void __launch_bounds__(256)
+upsample_argmax_nearest_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs,
+                               uint8_t* __restrict__ labels) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ int s_hsrc[kLabRows], s_wsrc[kLabCols];      // source row / column of each distinct slot
+  __shared__ int s_hslot[kLabRows], s_wslot[kLabCols];    // slot of each output row / column of the tile
+  __shared__ uint8_t s_lab[kLabRows][kLabCols];
+  const int n = blockIdx.z;
+  const int ho0 = blockIdx.y * kLabRows, wo0 = blockIdx.x * kLabCols;
+  const int nrows = min(kLabRows, Ho - ho0), ncols = min(kLabCols, Wo - wo0);
+  const int t = threadIdx.x;
+  const bool up_h = Hi <= Ho, up_w = Wi <= Wo;
+  const int hs0 = nearest_src(ho0, Hi, Ho), ws0 = nearest_src(wo0, Wi, Wo);
+  if (t < ncols) {
+    const int ws = nearest_src(wo0 + t, Wi, Wo);
+    const int slot = up_w ? ws - ws0 : t;
+    s_wslot[t] = slot;
+    s_wsrc[slot] = ws;  // upsampling: threads of one slot write the same value
+  }
+  if (t < nrows) {
+    const int hs = nearest_src(ho0 + t, Hi, Ho);
+    const int slot = up_h ? hs - hs0 : t;
+    s_hslot[t] = slot;
+    s_hsrc[slot] = hs;
+  }
+  __syncthreads();
+  const int srows = up_h ? nearest_src(ho0 + nrows - 1, Hi, Ho) - hs0 + 1 : nrows;
+  const int scols = up_w ? nearest_src(wo0 + ncols - 1, Wi, Wo) - ws0 + 1 : ncols;
+  for (int i = t; i < srows * scols; i += blockDim.x) {
+    const int r = i / scols, c = i - r * scols;
+    const __half* px = x + ((static_cast<size_t>(n) * Hi + s_hsrc[r]) * Wi + s_wsrc[c]) * xcs;
+    float best = -INFINITY;
+    int arg = 0;
+    for (int k = 0; k < C; ++k) {
+      const float v = __half2float(px[k]);
+      if (v > best) {
+        best = v;
+        arg = k;
+      }
+    }
+    s_lab[r][c] = static_cast<uint8_t>(arg);
+  }
+  __syncthreads();
+  const int r = t / (kLabCols / 8);
+  const int c0 = (t % (kLabCols / 8)) * 8;
+  if (r >= nrows || c0 >= ncols) return;
+  const uint8_t* lab = s_lab[s_hslot[r]];
+  uint8_t* dst = labels + (static_cast<size_t>(n) * Ho + ho0 + r) * Wo + wo0 + c0;
+  if (c0 + 8 <= ncols && (reinterpret_cast<uintptr_t>(dst) & 7) == 0) {
+    uint32_t lo = 0, hi = 0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      lo |= static_cast<uint32_t>(lab[s_wslot[c0 + j]]) << (8 * j);
+      hi |= static_cast<uint32_t>(lab[s_wslot[c0 + 4 + j]]) << (8 * j);
+    }
+    *reinterpret_cast<uint2*>(dst) = make_uint2(lo, hi);
+  } else {
+    for (int j = 0; j < 8 && c0 + j < ncols; ++j) dst[j] = lab[s_wslot[c0 + j]];
+  }
+}
+
+int upsample_argmax_nearest_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, uint8_t* labels,
+                                   cudaStream_t stream) {
+  const dim3 grid((Wo + kLabCols - 1) / kLabCols, (Ho + kLabRows - 1) / kLabRows, N);
+  FSB_LAUNCH(upsample_argmax_nearest_kernel, grid, dim3(256), 0, stream, N, C, Hi, Wi, Ho, Wo, static_cast<const __half*>(x), xcs,
+             labels);
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "upsample_argmax_nearest launch");
+  return FSB_OK;
+}
+
+// ------------------------------------------------------------------------------------------
 // layout plumbing
 // ------------------------------------------------------------------------------------------
 template <typename TIn>

@@ -14,7 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import (ConvDesc, FSB_ACT_IN_F32, FSB_CONV_AFFINE, FSB_CONV_FORCE_DIRECT, FSB_CONV_OUT_F32, FSB_CONV_RELU,
-                   FSB_CONV_STATS, check)
+                   FSB_CONV_STATS, FSB_CONV_X_DOWN2, FSB_CONV_Y_UP2, check)
 
 
 _raw_stream = getattr(torch._C, "_cuda_getCurrentRawStream", None)
@@ -156,18 +156,26 @@ def rowsum(rows):
 
 
 def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=False, out=None, off=(0, 0),
-             stats=None, force_direct=False, out_f32=False, stats_off=0):
+             stats=None, force_direct=False, out_f32=False, stats_off=0, down2=False, up2=False):
     """y = act(conv(x) * scale + shift); x/out NHWC fp16 views (see module docstring).  out_f32: fp32 NHWC output (the
     training path's raw conv result, normalised by BatchNorm from un-rounded values).  stats: a `conv_stats_buffer`; this
-    conv's per-channel sums land at column stats_off + c, its sums of squares at SC + stats_off + c of every row."""
+    conv's per-channel sums land at column stats_off + c, its sums of squares at SC + stats_off + c of every row.
+    down2: the conv runs on nearest(x, (H/2, W/2)), read in place from x (even H, W; stride 1).  up2: the result is
+    nearest(y, (2Ho, 2Wo)), written in place (out is the 2Ho x 2Wo map).  Both are bit for bit the separate resize."""
     N, Cin, H, W, xcs = nhwc_info(x)
+    if down2:
+        if H % 2 or W % 2:
+            raise ValueError("down2 needs an even input size, got %dx%d" % (H, W))
+        H, W = H // 2, W // 2
     Ho, Wo = conv_out_size(H, W, ksize, stride, pad, 1, off[0], off[1])
     odt = torch.float32 if out_f32 else torch.float16
+    up = 2 if up2 else 1
     if out is None:
-        out = empty_nhwc(N, Cout, Ho, Wo, x.device, dtype=odt)
+        out = empty_nhwc(N, Cout, Ho * up, Wo * up, x.device, dtype=odt)
     No, Co, Hy, Wy, ycs = nhwc_info(out, odt)
-    assert (No, Co, Hy, Wy) == (N, Cout, Ho, Wo), ((No, Co, Hy, Wy), (N, Cout, Ho, Wo))
+    assert (No, Co, Hy, Wy) == (N, Cout, Ho * up, Wo * up), ((No, Co, Hy, Wy), (N, Cout, Ho * up, Wo * up))
     flags = (FSB_CONV_RELU if relu else 0) | (FSB_CONV_AFFINE if (scale is not None or shift is not None) else 0)
+    flags |= (FSB_CONV_X_DOWN2 if down2 else 0) | (FSB_CONV_Y_UP2 if up2 else 0)
     if stats is not None:
         flags |= FSB_CONV_STATS
     if force_direct:
@@ -296,6 +304,43 @@ def upsample_argmax(x, size, out=None):
     if out is None:
         out = torch.empty((N, Ho, Wo), device=x.device, dtype=torch.uint8)
     check(_lib.lib().fsb_upsample_argmax(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(out), _stream()), "fsb_upsample_argmax")
+    return out
+
+
+def nearest(x, size, out=None):
+    """F.interpolate(x, size, mode='nearest') on NHWC fp16 views (torch's legacy index rule; a copy, so bit-exact)"""
+    N, Cc, Hi, Wi, xcs = nhwc_info(x)
+    Ho, Wo = int(size[0]), int(size[1])
+    if out is None:
+        out = empty_nhwc(N, Cc, Ho, Wo, x.device)
+    _, Co, Hy, Wy, ycs = nhwc_info(out)
+    assert (Co, Hy, Wy) == (Cc, Ho, Wo)
+    check(_lib.lib().fsb_nearest_fwd(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(out), ycs, _stream()), "fsb_nearest_fwd")
+    return out
+
+
+def upsample_logits_nearest(x, size, dtype=torch.float32, out=None):
+    """NHWC fp16 logits -> NCHW (contiguous) logits at `size`, mode='nearest'."""
+    N, Cc, Hi, Wi, xcs = nhwc_info(x)
+    Ho, Wo = int(size[0]), int(size[1])
+    if out is None:
+        out = torch.empty((N, Cc, Ho, Wo), device=x.device, dtype=dtype)
+    assert out.is_contiguous() and out.dtype in (torch.float16, torch.float32) and tuple(out.shape) == (N, Cc, Ho, Wo)
+    check(_lib.lib().fsb_upsample_logits_nearest_nchw(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(out),
+                                                      int(out.dtype == torch.float32), _stream()),
+          "fsb_upsample_logits_nearest_nchw")
+    return out
+
+
+def upsample_argmax_nearest(x, size, out=None):
+    """uint8 argmax over classes of upsample_logits_nearest(x, size), without materialising the logits"""
+    N, Cc, Hi, Wi, xcs = nhwc_info(x)
+    Ho, Wo = int(size[0]), int(size[1])
+    if out is None:
+        out = torch.empty((N, Ho, Wo), device=x.device, dtype=torch.uint8)
+    assert out.is_contiguous() and out.dtype == torch.uint8 and tuple(out.shape) == (N, Ho, Wo)
+    check(_lib.lib().fsb_upsample_argmax_nearest(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(out), _stream()),
+          "fsb_upsample_argmax_nearest")
     return out
 
 

@@ -2,10 +2,14 @@
 
     cd <FasterSeg>/search && python -m fasterseg_b200.launch train_search.py
     torchrun --nproc-per-node 8 -m fasterseg_b200.launch train_search.py        # data parallel
+    cd <FasterSeg>/latency && python -m fasterseg_b200.launch run_latency.py
 
-The reference resolves `operations`, `slimmable_ops`, `seg_oprs`, `model_seg`, `model_search`, `genotypes` from cwd
-(search/model_search.py:4-9, train/train.py:32); registering our modules under those names in `sys.modules` BEFORE the
-script imports them swaps the whole L1/L2 layer with zero script edits (SURVEY section 8b).  The shim also applies the
+The reference resolves `operations`, `slimmable_ops`, `seg_oprs`, `model_seg`, `model_search`, `genotypes` from the script's
+directory (search/model_search.py:4-9, train/train.py:32); registering our modules under those names in `sys.modules` BEFORE the
+script imports them swaps the whole L1/L2 layer with zero script edits (SURVEY section 8b).  The three directories hold
+different copies: for a script in a directory named `latency`, `operations` and `model_seg` are the latency/ deployment
+network (fasterseg_b200.latency_variant: nearest resizes, single-conv stride-2 FactorizedReduce) that run_latency.py builds and
+times; every other directory gets the train/ modules.  The shim also applies the
 py3.12 / torch 2.x compat patches the old scripts need (SURVEY section 5 "compat list") and, under torchrun, the
 data-parallel hooks of `fasterseg_b200.parallel`.
 """
@@ -20,9 +24,19 @@ import types
 SHADOWED = ("genotypes", "slimmable_ops", "operations", "seg_oprs", "model_seg", "model_search")
 
 
-def install_shadow_modules():
-    for name in SHADOWED:
-        sys.modules[name] = importlib.import_module("fasterseg_b200." + name)
+LATENCY_VARIANT = ("operations", "model_seg")   # modules of latency/ that differ from train/
+
+
+def shadow_module_names(script=None):
+    """{module name the script imports: our module} -- the latency/ variant for a script whose directory is named `latency`"""
+    latency = script is not None and os.path.basename(os.path.dirname(os.path.abspath(script))) == "latency"
+    return {name: "fasterseg_b200." + ("latency_variant." + name if latency and name in LATENCY_VARIANT else name)
+            for name in SHADOWED}
+
+
+def install_shadow_modules(script=None):
+    for name, target in shadow_module_names(script).items():
+        sys.modules[name] = importlib.import_module(target)
     return [sys.modules[n] for n in SHADOWED]
 
 
@@ -209,12 +223,12 @@ def main(argv=None):
         raise SystemExit("usage: python -m fasterseg_b200.launch <reference_script.py> [args...]")
     from . import _lib
     _lib.lib()  # fail loudly up front if the native library has not been built
+    script = argv[0]
     install_compat_patches()
-    install_shadow_modules()
+    install_shadow_modules(script)
     install_data_parallel()
     from . import optim
     optim.install()      # torch.optim.SGD / nn.utils.clip_grad_norm_ take the flat path after a captured `_loss` (torch's otherwise)
-    script = argv[0]
     sys.argv = argv
     sys.path.insert(0, os.path.dirname(os.path.abspath(script)) or ".")
     runpy.run_path(script, run_name="__main__")

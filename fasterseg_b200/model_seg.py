@@ -64,6 +64,8 @@ class Cell(nn.Module):
 
 
 class Network_Multi_Path_Infer(nn.Module):
+    _cell_cls = Cell   # the latency/ variant (latency_variant/model_seg.py) builds its cells from its own operators
+
     def __init__(self, alphas, betas, ratios, num_classes=19, layers=9, criterion=nn.CrossEntropyLoss(ignore_index=-1),
                  Fch=12, width_mult_list=[1., ], stem_head_width=(1., 1.), ignore_skip=False):
         super(Network_Multi_Path_Infer, self).__init__()
@@ -156,7 +158,7 @@ class Network_Multi_Path_Infer(nn.Module):
                 if layer < len(paths[lead]) - 1:
                     assert down == paths[lead][layer + 1] - paths[lead][layer]
                 c_in, c_out = self._cell_channels(lead, layer)
-                cell = Cell(ops[lead][layer], c_in, c_out, down)
+                cell = self._cell_cls(ops[lead][layer], c_in, c_out, down)
                 if down:   # the feature entering a down-sampling cell is what the refine conv of the finer scale concatenates
                     stride = 2 ** (paths[lead][layer] + 3)
                     for b in members:

@@ -224,7 +224,7 @@ class _Residual(_Primitive):
         h_out, w_out = self._out_hw(h_in, w_in)
         name = "%s_H%d_W%d_Cin%d_Cout%d_stride%d_dilation%d" % (self._table_prefix, h_in, w_in, c_in, c_out, self.stride,
                                                                self.dilation)
-        measure_cls = OPS_Class_by_prefix[self._table_prefix]
+        measure_cls = self._measure_classes[self._table_prefix]
         latency = _table_latency(name, lambda: measure_cls._latency(h_in, w_in, c_in, c_out, self.kernel_size, self.stride,
                                                                     self.dilation, self.groups))
         return latency, (c_out, h_out, w_out)
@@ -400,3 +400,4 @@ OPS_Class['conv_2x_downup'] = BasicResidual_downup_2x
 # the reference measures a missing downup_2x table entry with BasicResidual2x._latency (operations.py:430)
 OPS_Class_by_prefix = {"BasicResidual1x": BasicResidual1x, "BasicResidual_downup_1x": BasicResidual_downup_1x,
                        "BasicResidual2x": BasicResidual2x}
+_Residual._measure_classes = OPS_Class_by_prefix   # a network variant with other operator classes measures with its own

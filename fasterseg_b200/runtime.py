@@ -7,6 +7,7 @@ replay of frame i and the D2H copy of frame i-1 on three streams.
 """
 from __future__ import annotations
 
+import collections
 from typing import List, Optional
 
 import torch
@@ -44,6 +45,7 @@ class LaunchCounter:
 
     def __init__(self):
         self.n = 0
+        self.by_name = collections.Counter()   # launches per C-ABI call name (e.g. "fsb_conv_fwd")
         self._orig = None
 
     def __enter__(self):
@@ -53,6 +55,7 @@ class LaunchCounter:
 
         def counting_check(rc, what=""):
             counter.n += 1
+            counter.by_name[what] += 1
             return counter._orig(rc, what)
 
         F_.check = counting_check

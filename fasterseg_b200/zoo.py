@@ -27,9 +27,16 @@ def objective_acc_lat(acc, lat, lat_target=8.3, alpha=-0.07, beta=-0.07):
     return acc * math.pow(lat / lat_target, alpha if lat <= lat_target else beta)
 
 
-def build_network(arch_idx=1, lasts=None, training=False, num_classes=19, layers=16, Fch=12):
-    """Network_Multi_Path_Infer for a shipped genotype, constructed as train/train.py:95-105 does."""
-    from .model_seg import Network_Multi_Path_Infer
+def build_network(arch_idx=1, lasts=None, training=False, num_classes=19, layers=16, Fch=12, variant="train"):
+    """Network_Multi_Path_Infer for a shipped genotype, constructed as train/train.py:95-105 does.
+    variant: "train" (the train/ network: bilinear resizes) or "latency" (the latency/ deployment network: nearest resizes,
+    single-conv stride-2 FactorizedReduce; inference only -- latency_variant/)."""
+    if variant == "train":
+        from .model_seg import Network_Multi_Path_Infer
+    elif variant == "latency":
+        from .latency_variant.model_seg import Network_Multi_Path_Infer
+    else:
+        raise ValueError("variant must be 'train' or 'latency', got %r" % (variant,))
     state = load_arch(arch_idx)
     model = Network_Multi_Path_Infer(
         [state["alpha_%d_0" % arch_idx], state["alpha_%d_1" % arch_idx], state["alpha_%d_2" % arch_idx]],

@@ -46,6 +46,15 @@ typedef enum fsb_status {
 #define FSB_ACT_IN_F32 32u      /* fsb_affine_act: x is fp32 NHWC */
 #define FSB_CONV_STATS 8u       /* also produce per-channel sum / sum-of-squares of the (pre-affine) fp32 conv output as
                                    PARTIAL ROWS, one per CTA (BN train, K2) -- see "Deterministic statistics" below */
+/* Nearest-neighbour resizes folded into the tensor maps of the wgmma conv (latency/ deployment network,
+ * latency/operations.py:265,269,427,434, latency/model_seg.py:305,309,315).  Addresses change, nothing else: the result is
+ * bit for bit the conv of the resized input / the resized conv output. */
+#define FSB_CONV_X_DOWN2 64u    /* x is a 2H x 2W map (pixel stride x_cstride); the conv reads its even rows and columns, i.e.
+                                   F.interpolate(x, (H, W), mode='nearest'); H, W in the desc are the HALF size. Stride 1 only */
+#define FSB_CONV_Y_UP2 128u     /* y is a 2Ho x 2Wo map (pixel stride y_cstride); every output pixel is stored to its 2x2 block,
+                                   i.e. F.interpolate(conv, (2Ho, 2Wo), mode='nearest').  Needs the TMA-store epilogue: fp16
+                                   output, Cout and y_cstride multiples of 8, 16-byte aligned y, Cin >= 16; not with
+                                   FSB_CONV_STATS / FSB_CONV_OUT_F32 / FSB_CONV_FORCE_DIRECT (FSB_ERR_UNSUPPORTED) */
 
 /* One convolution launch.  Replaces F.conv2d at search/slimmable_ops.py:47 and every nn.Conv2d in
  * search/operations.py:42-534 / search/seg_oprs.py:17-39,228-274, fused with the BatchNorm (eval) +
@@ -173,6 +182,20 @@ int fsb_upsample_logits_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const
  * torch.argmax / np.argmax at tools/engine/evaluator.py:315-318). */
 int fsb_upsample_argmax(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, uint8_t* labels,
                         void* stream);
+/* F.interpolate(mode='nearest') (torch's legacy rule, not 'nearest-exact') on fp16 NHWC channel slices (latency/ network,
+ * latency/operations.py:265,269,427,434, latency/model_seg.py:305,309,315).  Per axis
+ *   src = min((int)floorf((float)dst * ((float)in / (float)out)), in - 1)   in fp32, exactly as torch computes it.
+ * C, strides multiples of 8, pointers 16-byte aligned.  No ReLU flag: a copy commutes with ReLU, apply it in the producer. */
+int fsb_nearest_fwd(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, void* y, int y_cstride,
+                    void* stream);
+/* Final x8 logits upsample of the latency/ network (latency/model_seg.py:362) with the same index rule: NHWC fp16 -> NCHW
+ * (out_dtype 0 = fp16, 1 = fp32), 16-byte stores along W. */
+int fsb_upsample_logits_nearest_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, void* y,
+                                     int out_dtype, void* stream);
+/* argmax over classes of fsb_upsample_logits_nearest_nchw's output -> uint8 labels [N, Ho, Wo], first maximum wins; the argmax
+ * is taken once per source pixel and replicated. */
+int fsb_upsample_argmax_nearest(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, uint8_t* labels,
+                                void* stream);
 /* NCHW (fp32 or fp16) -> NHWC fp16 and back; plumbing for callers that hand us reference-layout tensors. */
 int fsb_nchw_to_nhwc_f16(int N, int C, int H, int W, const void* x, int x_is_f32, void* y, int y_cstride,
                          void* stream);

@@ -11,6 +11,9 @@ doubling protocol of tools/utils/darts_utils.py:182-223 instead, ~7 s per entry)
 
   python tools/build_latency_table.py --out latency_lookup_table.npy            # one pass over the 667 operator shapes
   python tools/build_latency_table.py --list                                    # print the keys only (no GPU needed)
+  python tools/build_latency_table.py --variant latency --out latency/latency_lookup_table.npy
+                                    # the same keys measured on the latency/ deployment network's operators (nearest resizes,
+                                    # single-conv stride-2 FactorizedReduce), from which the reference built its table
 
 `table_keys()` is checked on the build machine against the key set of the reference's shipped table
 (tests/test_latency_table_keys_cpu.py)."""
@@ -83,9 +86,20 @@ _PATTERNS = (
 )
 
 
-def build_module(key):
-    """-> (nn.Module in eval mode, input shape (1, C, H, W)) for a table key"""
-    from fasterseg_b200 import operations as ops
+def operators(variant="train"):
+    """the operator module a table is measured with: the train/ network's or the latency/ deployment network's"""
+    if variant == "latency":
+        from fasterseg_b200.latency_variant import operations as ops
+    elif variant == "train":
+        from fasterseg_b200 import operations as ops
+    else:
+        raise ValueError("variant must be 'train' or 'latency', got %r" % (variant,))
+    return ops
+
+
+def build_module(key, variant="train"):
+    """-> (nn.Module in eval mode, input shape (1, C, H, W)) for a table key, built from `operators(variant)`"""
+    ops = operators(variant)
     from fasterseg_b200.seg_oprs import FeatureFusion, Head
     for rx, kind in _PATTERNS:
         m = rx.match(key)
@@ -140,6 +154,8 @@ def main():
     ap.add_argument("--list", action="store_true", help="print the keys and exit (no GPU)")
     ap.add_argument("--protocol", default="fast", choices=["fast", "reference"])
     ap.add_argument("--limit", type=int, default=0, help="only the first N keys (smoke test)")
+    ap.add_argument("--variant", default="train", choices=["train", "latency"],
+                    help="operators to measure: train/ (bilinear) or latency/ (nearest, single-conv stride-2 skip)")
     args = ap.parse_args()
     keys = table_keys()
     if args.limit:
@@ -150,7 +166,7 @@ def main():
         return
     table = {}
     for i, key in enumerate(keys):
-        module, shape = build_module(key)
+        module, shape = build_module(key, args.variant)
         table[key] = float(time_module(module, shape, args.protocol))
         if i % 50 == 0:
             print("%4d/%d %-70s %.4f ms" % (i, len(keys), key, table[key]), flush=True)
