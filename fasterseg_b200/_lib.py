@@ -118,6 +118,9 @@ _SIGS = {
     "fsb_peer_begin": (C.c_int, [C.c_int, _P]),
     "fsb_peer_allreduce_f32": (C.c_int, [_P, C.c_int64, _P]),
     "fsb_peer_shutdown": (C.c_int, []),
+    "fsb_supernet_latency_workspace_bytes": (C.c_size_t, [_P]),
+    "fsb_supernet_latency_fwd": (C.c_int, [_P] * 13 + [_P]),
+    "fsb_supernet_latency_bwd": (C.c_int, [_P] * 12 + [_P]),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

@@ -594,6 +594,32 @@ def to_nchw(x, dtype=torch.float32):
     return call(ToNCHWFn, x, dtype)
 
 
+class SupernetLatencyFn(torch.autograd.Function):
+    """Network_Multi_Path.forward_latency (model_search.py:361-475) as K14: one launch forward, one backward.  Inputs the plan does
+    not differentiate arrive detached and get None, like the walk, which never puts them in the graph (Adam then skips them)."""
+
+    @staticmethod
+    def forward(ctx, plan, noise, diff, *params):
+        dev = noise.device
+        ws = torch.empty(F_.supernet_latency_workspace_bytes(plan.host) // 4, dtype=torch.float32, device=dev)
+        out = torch.empty((), dtype=torch.float32, device=dev)
+        F_.supernet_latency_fwd(plan.host, plan.on(dev), params, noise, ws, out)
+        ctx.plan, ctx.diff, ctx.ws = plan, diff, ws
+        ctx.shapes = [p.shape for p in params]
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        dev = gout.device
+        grads = [torch.empty(s, dtype=torch.float32, device=dev) if d else None for s, d in zip(ctx.shapes, ctx.diff)]
+        F_.supernet_latency_bwd(ctx.plan.host, ctx.plan.on(dev), gout.float().contiguous(), ctx.ws, grads)
+        return (None, None, None, *grads)
+
+
+def supernet_latency(plan, noise, params, diff):
+    return SupernetLatencyFn.apply(plan, noise, tuple(diff), *params)
+
+
 def weighted_sum(wts, xs):
     return call(WsumFn, wts, *xs)
 

@@ -274,6 +274,39 @@ def flat_sgd(block_map, nblocks, segs, live, G, M, lr, momentum, weight_decay):
                                   float(weight_decay), _stream()), "fsb_flat_sgd")
 
 
+def _f32_ptrs(ts, what):
+    for t in ts:
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or not _on_device(t)):
+            raise ValueError("%s: expected contiguous CUDA float32 tensors, got %s %s" % (what, t.dtype, tuple(t.shape)))
+    return [_ptr(t) for t in ts]
+
+
+def supernet_latency_workspace_bytes(plan_host: torch.Tensor) -> int:
+    """bytes of the caller-owned workspace that fsb_supernet_latency_fwd fills and _bwd reads (host math on the plan header)"""
+    assert plan_host.dtype == torch.int32 and not plan_host.is_cuda
+    n = int(_lib.lib().fsb_supernet_latency_workspace_bytes(_ptr(plan_host)))
+    if n == 0:
+        raise _lib.FsbError("fsb_supernet_latency_workspace_bytes: invalid plan")
+    return n
+
+
+def supernet_latency_fwd(plan_host, plan, params, noise, workspace, out):
+    """out[()] = expected latency of the supernet (K14).  params: the 8 arch logit tensors (alphas x3, betas x2, ratios x3), None where
+    the plan does not read them; noise: gumbel uniforms or forced width indices on the device; workspace: saved for the backward"""
+    assert len(params) == 8 and plan.dtype == torch.int32 and _on_device(plan)
+    ptrs = _f32_ptrs(list(params) + [noise, workspace, out], "fsb_supernet_latency_fwd")
+    check(_lib.lib().fsb_supernet_latency_fwd(_ptr(plan_host), _ptr(plan), *ptrs, _stream()), "fsb_supernet_latency_fwd")
+    return out
+
+
+def supernet_latency_bwd(plan_host, plan, gout, workspace, grads):
+    """grads: 8 tensors shaped like the arch logits (None where the plan does not differentiate), overwritten with d latency * gout"""
+    assert len(grads) == 8 and plan.dtype == torch.int32 and _on_device(plan)
+    ptrs = _f32_ptrs([gout, workspace] + list(grads), "fsb_supernet_latency_bwd")
+    check(_lib.lib().fsb_supernet_latency_bwd(_ptr(plan_host), _ptr(plan), *ptrs, _stream()), "fsb_supernet_latency_bwd")
+    return grads
+
+
 def bilinear(x, size, relu=False, out=None):
     N, Cc, Hi, Wi, xcs = nhwc_info(x)
     Ho, Wo = int(size[0]), int(size[1])

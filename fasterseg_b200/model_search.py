@@ -355,11 +355,23 @@ class Network_Multi_Path(nn.Module):
 
     def forward_latency(self, size, alpha=True, beta=True, ratio=True):
         """Expected latency of the current architecture distribution from the per-op lookup table
-        (model_search.py:361-475): scalar arithmetic on the arch parameters' device.  The recurrences below reproduce the
-        reference's, including which beta row weights the running totals (see `pending`)."""
+        (model_search.py:361-475).  With the arch parameters on CUDA and every reachable table entry present, one kernel
+        evaluates it (supernet_latency.py, K14) and one more differentiates it; otherwise `_latency_walk` runs as scalar
+        arithmetic on the arch parameters' device, measuring and persisting any missing table entry."""
+        from . import supernet_latency
+        mode = self._current_mode() if ratio else 'max'
+        if supernet_latency.usable(self):
+            plan = supernet_latency.plan_for(self, size, alpha, beta, ratio, mode)
+            if plan is not None:
+                return supernet_latency.expected_latency(self, plan)
         alphas, betas = self._distributions(alpha, beta)
-        ratios = self.sample_prun_ratio(mode=self._current_mode() if ratio else 'max')
+        ratios = self.sample_prun_ratio(mode=mode)
+        return self._latency_walk(size, alphas, betas, ratios, lambda cell, size, a, r: cell.forward_latency(size, a, r))
 
+    def _latency_walk(self, size, alphas, betas, ratios, cell_latency):
+        """The expected-latency recurrence over the trellis.  cell_latency(cell, size, alphas row, (in, out, down) ratios) ->
+        ((keep ms, size), (down ms, size) | None).  The recurrences reproduce the reference's, including which beta row weights
+        the running totals (see `settle`); supernet_latency.py traces this same code into the kernel's plan."""
         stem_ms = 0
         for block in self.stem[self.arch_idx]:
             ms, size = block.forward_latency(size)
@@ -394,12 +406,12 @@ class Network_Multi_Path(nn.Module):
             r = self._ratio_triple(node.layer, node.scale, ratios)
             if node.beta_row is None:
                 (src, port), = node.feeds
-                keep, down = cell.forward_latency(prev[src][port], a, r)
+                keep, down = cell_latency(cell, prev[src][port], a, r)
                 cur[node.scale] = (keep[1], down[1] if down is not None else None)
                 pending.append([keep[0], down[0] if down is not None else None])
             else:
                 b = betas[node.scale][node.beta_row]
-                runs = [cell.forward_latency(prev[src][port], a, r) if b[n] > 0 else (None, None)
+                runs = [cell_latency(cell, prev[src][port], a, r) if b[n] > 0 else (None, None)
                         for n, (src, port) in enumerate(node.feeds)]
                 (keep0, down0), (keep1, down1) = runs
                 assert (keep0 is None and keep1 is None) or keep0[1] == keep1[1]

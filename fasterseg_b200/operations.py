@@ -140,7 +140,8 @@ class ConvNorm(_Primitive):
         layer = ConvNorm(C_in, C_out, kernel_size, stride, padding, dilation, groups, bias, slimmable=False)
         return compute_latency(layer, (1, C_in, h, w))
 
-    def forward_latency(self, size):
+    def latency_key(self, size):
+        """(latency-table key, output size) of this op at the configured ratio for an input of `size` = (C, H, W)"""
         c_in, h_in, w_in = size
         if self.slimmable:
             assert c_in == int(self.C_in * self.ratio[0]), "c_in %d, self.C_in * self.ratio[0] %d" % (c_in, self.C_in * self.ratio[0])
@@ -150,9 +151,14 @@ class ConvNorm(_Primitive):
             c_out = self.C_out
         h_out, w_out = self._out_hw(h_in, w_in)
         name = "ConvNorm_H%d_W%d_Cin%d_Cout%d_kernel%d_stride%d" % (h_in, w_in, c_in, c_out, self.kernel_size, self.stride)
-        latency = _table_latency(name, lambda: ConvNorm._latency(h_in, w_in, c_in, c_out, self.kernel_size, self.stride,
+        return name, (c_out, h_out, w_out)
+
+    def forward_latency(self, size):
+        name, size_out = self.latency_key(size)
+        c_in, h_in, w_in = size
+        latency = _table_latency(name, lambda: ConvNorm._latency(h_in, w_in, c_in, size_out[0], self.kernel_size, self.stride,
                                                                  self.padding, self.dilation, self.groups, self.bias))
-        return latency, (c_out, h_out, w_out)
+        return latency, size_out
 
     def forward(self, x, out=None):
         assert x.size()[1] == self.C_in, "{} {}".format(x.size()[1], self.C_in)
@@ -218,16 +224,22 @@ class _Residual(_Primitive):
         layer = cls(C_in, C_out, kernel_size, stride, dilation, groups, slimmable=False)
         return compute_latency(layer, (1, C_in, h, w))
 
-    def forward_latency(self, size):
+    def latency_key(self, size):
+        """(latency-table key, output size) of this op at the configured ratio for an input of `size` = (C, H, W)"""
         c_in, h_in, w_in = size
         c_out = self._active_io(c_in)
         h_out, w_out = self._out_hw(h_in, w_in)
         name = "%s_H%d_W%d_Cin%d_Cout%d_stride%d_dilation%d" % (self._table_prefix, h_in, w_in, c_in, c_out, self.stride,
                                                                self.dilation)
+        return name, (c_out, h_out, w_out)
+
+    def forward_latency(self, size):
+        name, size_out = self.latency_key(size)
+        c_in, h_in, w_in = size
         measure_cls = self._measure_classes[self._table_prefix]
-        latency = _table_latency(name, lambda: measure_cls._latency(h_in, w_in, c_in, c_out, self.kernel_size, self.stride,
+        latency = _table_latency(name, lambda: measure_cls._latency(h_in, w_in, c_in, size_out[0], self.kernel_size, self.stride,
                                                                     self.dilation, self.groups))
-        return latency, (c_out, h_out, w_out)
+        return latency, size_out
 
     def forward(self, x, out=None):
         stages = self._stages()
@@ -319,7 +331,8 @@ class FactorizedReduce(_Primitive):
         layer = FactorizedReduce(C_in, C_out, stride, slimmable=False)
         return compute_latency(layer, (1, C_in, h, w))
 
-    def forward_latency(self, size):
+    def latency_key(self, size):
+        """(latency-table key, output size) of this op at the configured ratio for an input of `size` = (C, H, W)"""
         c_in, h_in, w_in = size
         if self.slimmable:
             assert c_in == int(self.C_in * self.ratio[0])
@@ -329,8 +342,13 @@ class FactorizedReduce(_Primitive):
             c_out = self.C_out
         h_out, w_out = self._out_hw(h_in, w_in)
         name = "FactorizedReduce_H%d_W%d_Cin%d_Cout%d_stride%d" % (h_in, w_in, c_in, c_out, self.stride)
-        latency = _table_latency(name, lambda: FactorizedReduce._latency(h_in, w_in, c_in, c_out, self.stride))
-        return latency, (c_out, h_out, w_out)
+        return name, (c_out, h_out, w_out)
+
+    def forward_latency(self, size):
+        name, size_out = self.latency_key(size)
+        c_in, h_in, w_in = size
+        latency = _table_latency(name, lambda: FactorizedReduce._latency(h_in, w_in, c_in, size_out[0], self.stride))
+        return latency, size_out
 
     def forward(self, x, out=None):
         if self.stride == 2:

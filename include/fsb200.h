@@ -401,6 +401,26 @@ int fsb_flat_scale(const void* map, int nblocks, const void* segs, const uint8_t
 int fsb_flat_sgd(const void* map, int nblocks, const void* segs, const uint8_t* live, const float* G, float* M, float lr, float momentum,
                  float weight_decay, void* stream);
 
+/* K14: the supernet's expected latency, search/model_search.py:361-475 (Network_Multi_Path.forward_latency, called three times per
+ * architect step by search/architect.py:60-74, then loss_latency.backward()), as one launch forward and one backward with no host
+ * synchronisation.  `plan` is the int32 walk description built by fasterseg_b200/supernet_latency.py (header, constants, MixedOp
+ * terms with their [5][n_w][n_w] latency slices, the settle recurrence as ADD / MUL instructions, CSR use lists); the kernels read
+ * the device copy `plan`, the host copy `plan_host` sizes the launch.  Arch parameters are one architecture's fp32 logits
+ * (alphas [L|L-1|L-2][5], betas [L-2|L-3][2], ratios [L-1|L-1|L-2][n_w]); a tensor the plan's flags do not use may be NULL.
+ *   noise : gumbel uniforms [ratio rows][n_w] (arch_ratio sampling), else the forced width index of every ratio row (as float).
+ *   fsb_supernet_latency_fwd : *out = expected latency (ms); saves what the backward needs in `workspace`
+ *                              (fsb_supernet_latency_workspace_bytes(plan_host) bytes, caller-owned, kept until the backward).
+ *   fsb_supernet_latency_bwd : d/d(logits) of *gout * latency, written (not accumulated) in full for every tensor the plan
+ *                              differentiates: alphas / betas through their softmax, ratios through the straight-through gumbel
+ *                              sample (model_search.py:13-43).  Deterministic (fixed summation order, no atomics). */
+size_t fsb_supernet_latency_workspace_bytes(const int32_t* plan_host);
+int fsb_supernet_latency_fwd(const int32_t* plan_host, const int32_t* plan, const float* alpha0, const float* alpha1, const float* alpha2,
+                             const float* beta1, const float* beta2, const float* ratio0, const float* ratio1, const float* ratio2,
+                             const float* noise, float* workspace, float* out, void* stream);
+int fsb_supernet_latency_bwd(const int32_t* plan_host, const int32_t* plan, const float* gout, const float* workspace, float* dalpha0,
+                             float* dalpha1, float* dalpha2, float* dbeta1, float* dbeta2, float* dratio0, float* dratio1, float* dratio2,
+                             void* stream);
+
 #ifdef __cplusplus
 }
 #endif

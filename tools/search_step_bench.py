@@ -3,8 +3,8 @@
   pretrain step (configs[2]): search/train_search.py:246-250 with C.pretrain=True -- _loss = 4 forwards (max, min, random,
                               random) + backward + clip_grad_norm_(5) + SGD step, batch 3 x 3 x 256 x 512 per GPU
   search step   (configs[4]): architect.step (first-order: _loss on the search batch + Adam on arch params, architect.py:42-76,
-                              latency term omitted: latency_weight[0] = 0 and the table lookups are scalar python) followed by the
-                              weight step, batch 2 x 3 x 224 x 448 per GPU
+                              latency term omitted; tools/architect_step_bench.py times the step with the student's latency
+                              term on the walk and on K14) followed by the weight step, batch 2 x 3 x 224 x 448 per GPU
 Synthetic data per SURVEY 8(d).  Prints one JSON line.
 Data parallel: launch with torchrun (--nproc-per-node N): per-rank shard of the same per-GPU batch (weak scaling), SyncBN
 statistics + end-of-backward gradient all-reduce (fasterseg_b200/parallel.py); the time is the max over ranks."""
