@@ -46,6 +46,7 @@ _SIGS = {
     "fsb_get_option": (C.c_int, [C.c_char_p]),
     "fsb_conv_kernel_id": (C.c_int, [C.POINTER(ConvDesc), _P, C.c_int]),
     "fsb_conv_stats_rows": (C.c_int, [C.POINTER(ConvDesc)]),
+    "fsb_conv_residency": (C.c_int, [C.POINTER(ConvDesc)]),
     "fsb_stat_rows": (C.c_int, [C.c_int64]),
     "fsb_wsum_rows": (C.c_int, [C.c_int64, C.c_int]),
     "fsb_rowsum": (C.c_int, [C.c_int, _P, C.c_int, C.c_int, _P, _P]),

@@ -213,6 +213,15 @@ int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats) {
   (void)with_stats;
   return conv_tc_strip(d) ? 2 : 1;
 }
+int fsb_conv_residency(const fsb_conv_desc* d) {
+  int rc = check_desc(d);
+  if (rc) return rc;
+  if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_residency: the descriptor runs on the direct kernel");
+  int ctas = 0;
+  rc = conv_tc_launch(d, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, true, &ctas);
+  return rc ? rc : ctas;
+}
 int fsb_stat_rows(int64_t pixels) { return stat_rows(pixels); }
 int fsb_wsum_rows(int64_t pixels, int C) { return wsum_rows(pixels, C); }
 int fsb_rowsum(int L, const float* src, int rows, int stride, float* out, void* stream) {

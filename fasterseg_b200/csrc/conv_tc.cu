@@ -14,7 +14,8 @@
 //   B tile  : packed fp16 weights [tap][Npad][Kpad] (K-major), one TMA box {BK, NT, 1}.
 //   D       : fp32 accumulator in the registers of one warpgroup (two m64 halves of the 128-pixel tile, NT <= 128
 //             columns each: at most 128 accumulator registers per thread).
-// Warp roles (256 threads): warp 0 = TMA producer (warps 1-3 only join the final barrier), warps 4-7 = the MMA warpgroup.
+// Warp roles (160 threads): warps 0-3 = the MMA warpgroup (wgmma needs a warpgroup starting at a warp index divisible by 4),
+// warp 4 = TMA producer.  No idle warps: registers are allocated per CTA at the kernel's count, so every idle warp costs residency.
 // After the main loop the warpgroup parks the accumulator in shared memory as [channel][pixel] and runs the epilogue on it
 // (BN scale/shift -> ReLU -> fp16 -> NHWC store with channel offset/stride, which is how torch.cat(dim=1) call sites
 // become free), one pixel per thread.
@@ -25,7 +26,8 @@ namespace fsb {
 
 constexpr int kTileM = 128;
 constexpr int kMaxStages = 8;
-constexpr int kThreads = 256;
+constexpr int kMmaThreads = 128;  // warps 0-3
+constexpr int kThreads = kMmaThreads + 32;
 constexpr int kAccLd = kTileM + 4;  // padded channel column of the parked accumulator: conflict-free fragment stores and row reads
 
 struct ConvTcParams {
@@ -121,7 +123,8 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
   const int n0 = blockIdx.y * NT;
   const int k_iters = p.taps * p.k_chunks;
 
-  if (warp == 0 && lane == 0) {
+  constexpr int kProducer = kMmaThreads / 32;
+  if (warp == kProducer && lane == 0) {
     tma_prefetch_desc(&p.tmap_a[0]);
     tma_prefetch_desc(&p.tmap_b);
     for (int s = 0; s < p.stages; ++s) {
@@ -144,7 +147,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
   }
   __syncthreads();
 
-  if (WIN && warp == 0) {
+  if (WIN && warp == kProducer) {
     // ================= TMA producer, window mode: one input window per chunk, one weight tile per (chunk, tap) =================
     uint8_t* bring = smem + 2 * p.win_stride;
     const uint32_t win_bytes = static_cast<uint32_t>(p.win_rows * p.win_pitch) * 128u;
@@ -167,7 +170,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
         rp.advance(p.stages);
       }
     }
-  } else if (warp == 0) {
+  } else if (warp == kProducer) {
     // ================= TMA producer (converged warp, one elected lane issues) =================
     RingPos rp;
     uint8_t* sa = smem;
@@ -189,9 +192,9 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
         if (rp.s == 0) sa = smem;
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // ================= MMA warpgroup: wgmma over the stage ring, one stage in flight behind the current one =================
-    const int tw = threadIdx.x - 128;  // thread index inside the warpgroup
+    const int tw = threadIdx.x;  // thread index inside the warpgroup
     float acc[2][NT / 2];
 #pragma unroll
     for (int h = 0; h < 2; ++h)
@@ -280,7 +283,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
     named_bar_sync(1, 128);
 
     // ================= epilogue: thread m of the warpgroup owns pixel m of the tile =================
-    const int q = warp & 3;
+    const int q = warp;
     const int m = q * 32 + lane;
     const int oh = h0 + m / p.tw;
     const int ow = w0 + m % p.tw;
@@ -384,7 +387,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
       if (p.tma_store) {
         fence_proxy_async_smem();           // generic-proxy smem writes -> visible to the TMA engine
         named_bar_sync(1, 128);             // the 4 epilogue warps
-        if (warp == 4 && lane == 0) {
+        if (threadIdx.x == 0) {
           const bool full = (NT - c0) >= 64;
           tma_store_4d(&p.tmap_y[full ? 0 : 1], smem + static_cast<size_t>(c0 >> 6) * (kTileM * 128), n0 + c0, w0, h0, img);
           if constexpr (UP2)
@@ -395,13 +398,13 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
         }
       }
     }  // 64-column batch
-    if (p.tma_store && warp == 4 && lane == 0) tma_store_wait_read();  // smem must outlive the bulk reads
+    if (p.tma_store && threadIdx.x == 0) tma_store_wait_read();  // smem must outlive the bulk reads
     if (do_stats) {
       // no atomics: the four warp partials are added in warp order and written as this tile's partial row; the consumer
       // (bn_finalize / rowsum) adds the rows in index order, so the statistics are bit-reproducible run to run
       named_bar_sync(2, 128);
       float* row = p.stats + static_cast<size_t>(blockIdx.x) * 2 * p.stats_C + p.stats_off;
-      for (int ch = static_cast<int>(threadIdx.x) - 128; ch < NT; ch += 128) {
+      for (int ch = static_cast<int>(threadIdx.x); ch < NT; ch += kMmaThreads) {
         if (n0 + ch >= p.Cout) continue;
         float a = s_stat[0 * NT + ch], b = s_stat[1 * NT + ch];
 #pragma unroll
@@ -417,14 +420,17 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
   __syncthreads();
 }
 
+// CTAs per SM each instance is compiled for (registers) and conv_tc_launch sizes its shared memory for
+__host__ __device__ constexpr int conv_tc_residency(int nt) { return nt <= 64 ? 3 : 2; }
+
 template <int BK, int NT, bool WIN>
-__global__ void __launch_bounds__(kThreads, NT <= 64 ? 2 : 1)
+__global__ void __launch_bounds__(kThreads, conv_tc_residency(NT))
 conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
   conv_tc_body<BK, NT, WIN, false>(p, nullptr, 1);
 }
 
 template <int BK, int NT, bool WIN>
-__global__ void __launch_bounds__(kThreads, NT <= 64 ? 2 : 1)
+__global__ void __launch_bounds__(kThreads, conv_tc_residency(NT))
 conv_tc_up2_kernel(const __grid_constant__ ConvTcUp2Params q) {
   conv_tc_body<BK, NT, WIN, true>(q.p, q.tmap_up, q.y_reps);
 }
@@ -508,31 +514,39 @@ int conv_tc_supported(const fsb_conv_desc* d) {
   return 1;
 }
 
+// residency != nullptr: store the CTAs per SM the instance reaches with smem_bytes of dynamic shared memory instead of launching
 template <int BK, int NT, bool WIN = false>
-static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q) {
+static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q, int* residency) {
   const bool up2 = q.y_reps > 1;
   const void* kernel = up2 ? reinterpret_cast<const void*>(conv_tc_up2_kernel<BK, NT, WIN>)
                            : reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, WIN>);
   if (int rc = ensure_dyn_smem(kernel, 220 * 1024, "cudaFuncSetAttribute(conv_tc)")) return rc;
+  if (residency) {
+    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(residency, kernel, kThreads, smem_bytes);
+    return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_tc)");
+  }
   const cudaError_t e = up2 ? launch_kernel(conv_tc_up2_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, q)
                             : launch_kernel(conv_tc_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, q.p);
   return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
 }
 
 template <int BK, bool WIN>
-static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q) {
+static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q, int* residency) {
   switch (n_tile) {
-    case 16: return conv_tc_run<BK, 16, WIN>(grid, smem_bytes, stream, q);
-    case 32: return conv_tc_run<BK, 32, WIN>(grid, smem_bytes, stream, q);
-    case 48: return conv_tc_run<BK, 48, WIN>(grid, smem_bytes, stream, q);
-    case 64: return conv_tc_run<BK, 64, WIN>(grid, smem_bytes, stream, q);
-    case 96: return conv_tc_run<BK, 96, WIN>(grid, smem_bytes, stream, q);
-    default: return conv_tc_run<BK, 128, WIN>(grid, smem_bytes, stream, q);
+    case 16: return conv_tc_run<BK, 16, WIN>(grid, smem_bytes, stream, q, residency);
+    case 32: return conv_tc_run<BK, 32, WIN>(grid, smem_bytes, stream, q, residency);
+    case 48: return conv_tc_run<BK, 48, WIN>(grid, smem_bytes, stream, q, residency);
+    case 64: return conv_tc_run<BK, 64, WIN>(grid, smem_bytes, stream, q, residency);
+    case 96: return conv_tc_run<BK, 96, WIN>(grid, smem_bytes, stream, q, residency);
+    default: return conv_tc_run<BK, 128, WIN>(grid, smem_bytes, stream, q, residency);
   }
 }
 
+// static shared memory of an instance: the 2 * kMaxStages + 4 mbarriers and s_scale / s_shift of conv_tc_body
+static size_t conv_tc_static_smem(int n_tile) { return (2 * kMaxStages + 4) * 8 + static_cast<size_t>(n_tile) * 2 * 4; }
+
 int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu, bool window_ok) {
+                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu, bool window_ok, int* residency) {
   const ConvGeom g = conv_geom(d);
   if (cu && (d->stride != 1 || (d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS))))
     return set_error(FSB_ERR_INVALID, "conv_tc: custom tap tables need a stride-1 fp16 problem");
@@ -619,10 +633,15 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
 
   const size_t stage_bytes = (win ? 0 : static_cast<size_t>(kTileM) * bk * 2) + static_cast<size_t>(n_tile) * bk * 2;
   const int k_iters = p.taps * p.k_chunks;
-  // 128-channel tiles hold 128 accumulator registers per thread: one CTA per SM, give the pipeline (almost) the whole shared
-  // memory; the same when the grid has at most one CTA per SM anyway (and for the row strip, whose windows alone take 100 KB).
-  // Otherwise keep two CTAs per SM resident.
-  const size_t smem_budget = (n_tile == 128 || m_tiles * n_tiles <= sms || strip) ? 200 * 1024 : 100 * 1024;
+  // Residency res = the CTAs per SM the launch can use: at most what the instance's registers allow (conv_tc_residency) and at
+  // most what the grid fills (CTAs / SMs, rounded up).  A multi-wave conv is bound by how many CTAs overlap on an SM (DESIGN.md
+  // section 3.3); a grid of 1-2 CTAs per SM gains nothing from a third slot and keeps the deeper ring.  Budget of the windows +
+  // stage ring: one CTA per SM (and the row strip, whose windows alone take 100 KB) gets (almost) the whole shared memory;
+  // otherwise an SM's 227 KB shared by res CTAs, less each CTA's static shared memory, the 1 KB the driver reserves per CTA and
+  // the 1 KB of slack that aligns the ring.
+  const int grid_res = (m_tiles * n_tiles + sms - 1) / sms;
+  const int res = strip ? 1 : (grid_res < conv_tc_residency(n_tile) ? grid_res : conv_tc_residency(n_tile));
+  const size_t smem_budget = res <= 1 ? 200 * 1024 : 227 * 1024 / res - conv_tc_static_smem(n_tile) - 2 * 1024;
   const size_t win_bytes = win ? 2 * static_cast<size_t>(p.win_stride) : 0;   // two input windows ahead of the weight ring
   int stages = static_cast<int>((smem_budget - win_bytes) / stage_bytes);
   if (stages < 2) stages = 2;
@@ -633,6 +652,20 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
                            : n_tile == 48 ? conv_tc_epilogue_bytes<48>() : n_tile == 64 ? conv_tc_epilogue_bytes<64>()
                            : n_tile == 96 ? conv_tc_epilogue_bytes<96>() : conv_tc_epilogue_bytes<128>();
   size_t smem_bytes = (win_bytes + stage_bytes * stages > epi_bytes ? win_bytes + stage_bytes * stages : epi_bytes) + 1024;
+  // Allocate the whole budget, so that no more than res CTAs share an SM.  The registers of a 160-thread instance leave room for
+  // more (up to 4 CTAs per SM at 96 registers), and left that way the grids of at most one or two CTAs per SM measured slower
+  // than with 256-thread CTAs (DESIGN.md section 3.3).
+  if (smem_bytes < smem_budget + 1024) smem_bytes = smem_budget + 1024;
+  const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles));
+  auto run = [&]() {
+    if (win) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, q, residency);
+    if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, q, residency);
+    return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, q, residency);
+  };
+  if (residency) {  // the query needs only the instance and its shared memory, not the tensor maps
+    q.y_reps = (d->flags & FSB_CONV_Y_UP2) ? 4 : 1;
+    return run();
+  }
   // ---- TMA-store epilogue: fp16 output whose pixels start on 16 B and whose channel count is a multiple of 8 ----
   // FSB_CONV_Y_UP2: y is the 2Ho x 2Wo map and every output pixel goes to its 2x2 block (nearest x2 folded into the store):
   // four lattice maps, one per (row, column) parity, each with the pixel steps of the full map doubled; the epilogue stores
@@ -741,10 +774,7 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     int rc = encode_tiled(&p.tmap_b, wpacked, 3, dims, str, boxB, bk * 2);
     if (rc) return rc;
   }
-  const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles));
-  if (win) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, q);
-  if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, q);
-  return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, q);
+  return run();
 }
 
 }  // namespace fsb

@@ -101,9 +101,11 @@ struct ConvTcCustom {
 };
 int conv_tc_supported(const fsb_conv_desc* d);
 bool conv_tc_strip(const fsb_conv_desc* d);  // conv_tc runs d in row-strip mode
-// window_ok = false keeps a 3x3 stride-1 problem on the per-tap mode unless FSB_CONV_TC2 forces the window mode
+// window_ok = false keeps a 3x3 stride-1 problem on the per-tap mode unless FSB_CONV_TC2 forces the window mode;
+// residency != nullptr launches nothing and stores the CTAs per SM of the instance and shared memory the call would launch with
 int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr, bool window_ok = true);
+                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr, bool window_ok = true,
+                   int* residency = nullptr);
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride);
 int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
                          float gscale, cudaStream_t stream);

@@ -150,6 +150,10 @@ int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats);
 /* number of partial statistic rows fsb_conv_fwd writes for `d` with FSB_CONV_STATS (depends on the kernel it dispatches):
  * stats must hold rows * 2 * SC floats; every row's entries of this conv's channels are written (no zeroing needed). */
 int fsb_conv_stats_rows(const fsb_conv_desc* d);
+/* CTAs per SM of the conv_tc launch fsb_conv_fwd makes for `d` (with stats iff d->flags has FSB_CONV_STATS): the CUDA occupancy
+ * calculator's answer for the kernel instance and the dynamic shared memory the launcher picks.  Launches nothing.
+ * FSB_ERR_UNSUPPORTED when `d` runs on the CUDA-core direct kernel; other negative values are errors. */
+int fsb_conv_residency(const fsb_conv_desc* d);
 
 /* Stem conv reading the caller's NCHW tensor directly (fp32 if x_is_f32 else fp16), 3x3 stride 2 pad 1,
  * Cin = 3, fused BN(eval)+ReLU, fp16 NHWC out.  ConvNorm at train/model_seg.py:193, search/model_search.py:148.
