@@ -38,9 +38,8 @@ int sm_count() {
   return n;
 }
 
-static const char* const kOptNames[OPT_COUNT] = {"FSB_CONV_TC2", "FSB_TC2_R", "FSB_TC2_ASTAGES", "FSB_NO_TMA_STORE",
-                                                 "FSB_DGRAD_S2_DIRECT", "FSB_WGRAD_TC", "FSB_CONV_PERSIST", "FSB_PERSIST_OCC",
-                                                 "FSB_PERSIST_STAGES", "FSB_UPSAMPLE_V2", "FSB_DETERMINISTIC", "FSB_CONV_TC3", "FSB_CONV_TC4", "FSB_CONV_TC5", "FSB_CONV_KSPLIT", "FSB_CONV_NTILE_MIN"};
+static const char* const kOptNames[OPT_COUNT] = {"FSB_CONV_TC2", "FSB_DGRAD_S2_DIRECT", "FSB_WGRAD_TC", "FSB_UPSAMPLE_V2",
+                                                 "FSB_DETERMINISTIC"};
 static int g_opts[OPT_COUNT];
 static std::once_flag g_opts_once;
 static void load_opts() {
@@ -110,10 +109,8 @@ int nhwc_to_nchw_launch(int, int, int, int, const void*, int, void*, int, cudaSt
 int copy_channels_launch(int64_t, int, const void*, int, void*, int, cudaStream_t);
 int bn_fold_launch(int, const float*, const float*, const float*, const float*, float, const float*, float*, float*, cudaStream_t);
 int bn_stats_launch(int64_t, int, const void*, int, int, float*, cudaStream_t);
-int stat_rows(int64_t);
 int wsum_rows(int64_t, int);
 int rowsum_launch(int, const float*, int, int, float*, cudaStream_t);
-int conv_tc_m_tiles(const fsb_conv_desc*);
 int bn_finalize_launch(int, const float*, int, int, double, const float*, const float*, float, float, float*, float*, float*, float*,
                        float*, float*, cudaStream_t, long long* = nullptr, const fsb_bn_sel* = nullptr, const int* = nullptr, int = 0);
 int affine_act_launch(int64_t, int, const void*, int, const float*, const float*, void*, int, uint32_t, cudaStream_t,
@@ -203,24 +200,20 @@ int fsb_get_option(const char* name) {
 
 int fsb_conv_stats_rows(const fsb_conv_desc* d) {
   if (check_desc(d)) return 0;
-  if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d)) return stat_rows(static_cast<int64_t>(d->N) * d->Ho * d->Wo);
-  return conv_tc_m_tiles(d);
+  return conv_plan(d).stat_rows;
 }
 int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats) {
   if (check_desc(d)) return -1;
-  if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d)) return 0;
   (void)y;
   (void)with_stats;
-  return conv_tc_strip(d) ? 2 : 1;
+  return conv_plan(d).direct ? 0 : 1;
 }
 int fsb_conv_residency(const fsb_conv_desc* d) {
   int rc = check_desc(d);
   if (rc) return rc;
-  if ((d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d))
-    return set_error(FSB_ERR_UNSUPPORTED, "conv_residency: the descriptor runs on the direct kernel");
-  int ctas = 0;
-  rc = conv_tc_launch(d, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, true, &ctas);
-  return rc ? rc : ctas;
+  const ConvPlan plan = conv_plan(d);
+  if (plan.direct) return set_error(FSB_ERR_UNSUPPORTED, "conv_residency: the descriptor runs on the direct kernel");
+  return plan.rc ? plan.rc : conv_tc_occupancy(plan);
 }
 int fsb_stat_rows(int64_t pixels) { return stat_rows(pixels); }
 int fsb_wsum_rows(int64_t pixels, int C) { return wsum_rows(pixels, C); }
@@ -303,12 +296,10 @@ int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, con
   if (rc) return rc;
   if (!x || !wpacked || !y) return set_error(FSB_ERR_INVALID, "conv_fwd: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const bool direct = (d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d);
-  if (direct && (d->flags & (FSB_CONV_X_DOWN2 | FSB_CONV_Y_UP2)))
-    return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd: FSB_CONV_X_DOWN2 / FSB_CONV_Y_UP2 need the wgmma kernel (Cin >= 16, x_cstride % 8 == 0, "
-                                          "no FSB_CONV_FORCE_DIRECT)");
-  if (direct) return conv_direct_launch(d, x, wpacked, scale, shift, y, stats, st);
-  return conv_tc_launch(d, x, wpacked, scale, shift, y, stats, st);
+  const ConvPlan plan = conv_plan(d);
+  if (plan.rc) return plan.rc;
+  if (plan.direct) return conv_direct_launch(d, x, wpacked, scale, shift, y, stats, st);
+  return conv_tc_launch(plan, d, x, wpacked, scale, shift, y, stats, st);
 }
 
 int fsb_stem_conv_nchw(int N, int H, int W, int Cout, const void* x, int x_is_f32, const float* w, const float* scale,

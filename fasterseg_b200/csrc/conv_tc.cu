@@ -76,10 +76,8 @@ struct ConvTcUp2Params {
 
 // shared memory after the main loop: [0, kOutBytes) = statistics partials or the TMA-store staging slabs,
 // [kOutBytes, + NT * kAccLd * 4) = the parked accumulator; both reuse the (then idle) stage ring
-template <int NT>
-__host__ __device__ constexpr uint32_t conv_tc_out_bytes() { return static_cast<uint32_t>((NT + 63) / 64) * kTileM * 128; }
-template <int NT>
-__host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes() { return conv_tc_out_bytes<NT>() + static_cast<uint32_t>(NT) * kAccLd * 4; }
+__host__ __device__ constexpr uint32_t conv_tc_out_bytes(int nt) { return static_cast<uint32_t>((nt + 63) / 64) * kTileM * 128; }
+__host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes(int nt) { return conv_tc_out_bytes(nt) + static_cast<uint32_t>(nt) * kAccLd * 4; }
 
 // Window mode (WIN: 3x3 stride-1 dilation-1 convs without custom tap tables).  Per 64-channel chunk the producer loads the
 // (th + 2) x (tw + 2) input pixels the tile needs (halo included, out-of-image pixels and channels >= Cin zero-filled by TMA)
@@ -89,8 +87,7 @@ __host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes() { return conv_tc
 // per (chunk, tap), through the stage ring.  Every input byte of a tile crosses L2 -> SM about 1.4x per chunk instead of 9x.
 // Each m64 half of the 128-pixel tile must be 8 groups of 8 window-contiguous pixels at one stride:
 //   16 x 8 tiles: half h = the 8 x 8 block at columns 8h..8h+7, groups = tile rows (stride tw + 2 pixels);
-//   8 x 16 tiles: half h = tile rows 8h..8h+7, groups = tile rows (stride tw + 2 pixels);
-//   row strip (128 x 1 tiles, FSB_CONV_TC2=2): half h = pixels 64h..64h+63 of the row, groups 8 pixels apart.
+//   8 x 16 tiles: half h = tile rows 8h..8h+7, groups = tile rows (stride tw + 2 pixels).
 
 // The kernel body.  UP2 (FSB_CONV_Y_UP2) only adds the stores of each staged slab to lattices 1 .. y_reps - 1; it is compiled
 // into instances of its own (conv_tc_up2_kernel) so that the instances every other call runs keep their registers.
@@ -262,7 +259,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
     wgmma_wait<0>();
     // park the accumulator as [channel][pixel] behind the epilogue's output area (the stage ring is idle now: every load
     // has been consumed and every MMA has retired in all four warps once the barrier below is passed)
-    float* s_acc = reinterpret_cast<float*>(smem + conv_tc_out_bytes<NT>());
+    float* s_acc = reinterpret_cast<float*>(smem + conv_tc_out_bytes(NT));
     named_bar_sync(1, 128);
     if constexpr (WIN) {
       // this thread's fragment rows are row0 and row0 + 8 (8-row groups g0 and g0 + 1) of each half
@@ -420,7 +417,7 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
   __syncthreads();
 }
 
-// CTAs per SM each instance is compiled for (registers) and conv_tc_launch sizes its shared memory for
+// CTAs per SM each instance is compiled for (registers) and conv_plan sizes its shared memory for
 __host__ __device__ constexpr int conv_tc_residency(int nt) { return nt <= 64 ? 3 : 2; }
 
 template <int BK, int NT, bool WIN>
@@ -438,8 +435,8 @@ conv_tc_up2_kernel(const __grid_constant__ ConvTcUp2Params q) {
 // ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
-static int encode_tiled(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                        const uint32_t* box, int swizzle_bytes) {
+int encode_tiled(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box, int swizzle_bytes) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return set_error(FSB_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable");
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
@@ -469,11 +466,6 @@ static int encode_tiled(CUtensorMap* map, const void* base, int rank, const uint
   return FSB_OK;
 }
 
-int encode_tiled_generic(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                         const uint32_t* box, int swizzle_bytes) {
-  return encode_tiled(map, base, rank, dims, strides_bytes, box, swizzle_bytes);
-}
-
 static inline int floordiv(int a, int b) { return (a >= 0) ? a / b : -((-a + b - 1) / b); }
 
 ConvGeom conv_geom(const fsb_conv_desc* d) {
@@ -485,69 +477,20 @@ ConvGeom conv_geom(const fsb_conv_desc* d) {
   return g;
 }
 
-// Which conv_tc mode can run d (without custom tap tables).  3x3 stride-1 dilation-1 convs may use the window mode on their
-// 16 x 8 / 8 x 16 tiles: the per-tap mode moves every input byte of a tile from L2 to the SM nine times, and on large maps
-// L2 -> SM bandwidth, not HBM or the tensor cores, bounds the kernel (DESIGN.md section 3.3); conv_tc_launch takes it when the
-// grid has more CTAs than SMs.  FSB_CONV_TC2=0 forces the per-tap mode and 1 the window mode (for A/B measurements and tests);
-// FSB_CONV_TC2=2 selects the row strip (128 x 1 tiles, Cin % 64 == 0, no statistics), which is slower: its two 50 KB windows
-// allow one CTA per SM.
-enum ConvTcMode { kPerTap, kWindow, kStrip };
-static ConvTcMode conv_tc_mode(const fsb_conv_desc* d) {
-  if (d->ksize != 3 || d->stride != 1 || d->dil != 1) return kPerTap;
-  const int o = opt(OPT_CONV_TC2);
-  if (o == 0) return kPerTap;
-  if (o == 2 && d->Cin % 64 == 0 && !(d->flags & FSB_CONV_STATS)) return kStrip;
-  return kWindow;
-}
-bool conv_tc_strip(const fsb_conv_desc* d) { return conv_tc_mode(d) == kStrip; }
-
-// spatial tiles (= CTAs along M = partial statistic rows) of conv_tc
-int conv_tc_m_tiles(const fsb_conv_desc* d) {
-  if (conv_tc_strip(d)) return ((d->Wo + kTileM - 1) / kTileM) * d->Ho * d->N;
-  const int tw = d->Wo >= 16 ? 16 : 8, th = kTileM / tw;
-  return ((d->Wo + tw - 1) / tw) * ((d->Ho + th - 1) / th) * d->N;
-}
-
 int conv_tc_supported(const fsb_conv_desc* d) {
   if (d->Cin < 16 || (d->x_cstride % 8) != 0) return 0;
   if (!(d->ksize == 1 || d->ksize == 3) || !(d->stride == 1 || d->stride == 2)) return 0;
   return 1;
 }
 
-// residency != nullptr: store the CTAs per SM the instance reaches with smem_bytes of dynamic shared memory instead of launching
-template <int BK, int NT, bool WIN = false>
-static int conv_tc_run(dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q, int* residency) {
-  const bool up2 = q.y_reps > 1;
-  const void* kernel = up2 ? reinterpret_cast<const void*>(conv_tc_up2_kernel<BK, NT, WIN>)
-                           : reinterpret_cast<const void*>(conv_tc_kernel<BK, NT, WIN>);
-  if (int rc = ensure_dyn_smem(kernel, 220 * 1024, "cudaFuncSetAttribute(conv_tc)")) return rc;
-  if (residency) {
-    const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(residency, kernel, kThreads, smem_bytes);
-    return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_tc)");
-  }
-  const cudaError_t e = up2 ? launch_kernel(conv_tc_up2_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, q)
-                            : launch_kernel(conv_tc_kernel<BK, NT, WIN>, grid, dim3(kThreads), smem_bytes, stream, q.p);
-  return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
-}
-
-template <int BK, bool WIN>
-static int conv_tc_run_nt(int n_tile, dim3 grid, size_t smem_bytes, cudaStream_t stream, const ConvTcUp2Params& q, int* residency) {
-  switch (n_tile) {
-    case 16: return conv_tc_run<BK, 16, WIN>(grid, smem_bytes, stream, q, residency);
-    case 32: return conv_tc_run<BK, 32, WIN>(grid, smem_bytes, stream, q, residency);
-    case 48: return conv_tc_run<BK, 48, WIN>(grid, smem_bytes, stream, q, residency);
-    case 64: return conv_tc_run<BK, 64, WIN>(grid, smem_bytes, stream, q, residency);
-    case 96: return conv_tc_run<BK, 96, WIN>(grid, smem_bytes, stream, q, residency);
-    default: return conv_tc_run<BK, 128, WIN>(grid, smem_bytes, stream, q, residency);
-  }
-}
-
 // static shared memory of an instance: the 2 * kMaxStages + 4 mbarriers and s_scale / s_shift of conv_tc_body
 static size_t conv_tc_static_smem(int n_tile) { return (2 * kMaxStages + 4) * 8 + static_cast<size_t>(n_tile) * 2 * 4; }
 
-int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu, bool window_ok, int* residency) {
-  const ConvGeom g = conv_geom(d);
+// descriptor checks of conv_plan: the flag combinations no kernel runs
+static int conv_check_flags(const fsb_conv_desc* d, bool direct, const ConvTcCustom* cu) {
+  if (direct && (d->flags & (FSB_CONV_X_DOWN2 | FSB_CONV_Y_UP2)))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd: FSB_CONV_X_DOWN2 / FSB_CONV_Y_UP2 need the wgmma kernel (Cin >= 16, x_cstride % 8 == 0, "
+                                          "no FSB_CONV_FORCE_DIRECT)");
   if (cu && (d->stride != 1 || (d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS))))
     return set_error(FSB_ERR_INVALID, "conv_tc: custom tap tables need a stride-1 fp16 problem");
   if (cu && (d->flags & (FSB_CONV_X_DOWN2 | FSB_CONV_Y_UP2)))
@@ -556,70 +499,159 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
     return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_X_DOWN2 needs a stride-1 conv");
   if ((d->flags & FSB_CONV_Y_UP2) && (d->flags & (FSB_CONV_STATS | FSB_CONV_OUT_F32)))
     return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_Y_UP2 cannot be combined with FSB_CONV_STATS or FSB_CONV_OUT_F32");
-  if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(wpacked) & 15))
-    return set_error(FSB_ERR_INVALID, "conv_tc: x / wpacked must be 16-byte aligned");
-  ConvTcUp2Params q;
-  memset(&q, 0, sizeof(q));
-  ConvTcParams& p = q.p;
-  const ConvTcMode mode = cu ? kPerTap : conv_tc_mode(d);
-  const bool strip = mode == kStrip;
-  p.taps = cu ? cu->ntaps : g.taps;
-  p.Ho = cu ? cu->Ho : d->Ho;
-  p.Wo = cu ? cu->Wo : d->Wo;
-  p.tw = strip ? kTileM : (p.Wo >= 16 ? 16 : 8);
-  p.th = kTileM / p.tw;
-  p.tiles_w = (p.Wo + p.tw - 1) / p.tw;
-  p.tiles_h = (p.Ho + p.th - 1) / p.th;
-  for (int i = 0; i < 9; ++i) p.tap_widx[i] = i;
-  p.Cout = d->Cout;
+  return FSB_OK;
+}
+
+ConvPlan conv_plan(const fsb_conv_desc* d, const ConvTcCustom* cu, bool window_ok) {
+  ConvPlan pl = {};
+  pl.direct = (d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d);
+  pl.rc = conv_check_flags(d, pl.direct, cu);
+  if (pl.direct) {
+    pl.stat_rows = stat_rows(static_cast<int64_t>(d->N) * d->Ho * d->Wo);
+    return pl;
+  }
+  const ConvGeom g = conv_geom(d);
+  pl.up2 = (d->flags & FSB_CONV_Y_UP2) != 0;
+  pl.taps = cu ? cu->ntaps : g.taps;
+  pl.Ho = cu ? cu->Ho : d->Ho;
+  pl.Wo = cu ? cu->Wo : d->Wo;
+  pl.tw = pl.Wo >= 16 ? 16 : 8;
+  pl.th = kTileM / pl.tw;
+  pl.tiles_w = (pl.Wo + pl.tw - 1) / pl.tw;
+  pl.tiles_h = (pl.Ho + pl.th - 1) / pl.th;
+  pl.m_tiles = pl.tiles_w * pl.tiles_h * d->N;
+  pl.stat_rows = pl.m_tiles;  // one partial row per spatial tile
   // Output-channel tiling: N tiles of 16, 32, 48, 64, 96 or 128 channels (the wgmma N of the kernel instance; B boxes past npad
   // rows are zero-filled by TMA and the epilogue stores only channels < Cout): the fewest tiles of <= 128, each the smallest
   // instance that covers its share.  When the spatial tiling alone cannot fill the machine (small maps at 1/16, 1/32
-  // resolution), split N further so that more SMs pull operands from L2 in parallel.
+  // resolution), split N further, down to 32-channel tiles, so that more SMs pull operands from L2 in parallel (a CTA still
+  // walks every tap and channel chunk; the split spreads the weight loads and the epilogue over more SMs).
   static const int kNt[] = {16, 32, 48, 64, 96, 128};
-  const int m_tiles = p.tiles_w * p.tiles_h * d->N;
-  int n_tiles = (g.npad + 127) / 128;
+  pl.n_tiles = (g.npad + 127) / 128;
   int ni = 0;
-  while (kNt[ni] * n_tiles < g.npad) ++ni;
-  int n_tile = kNt[ni];
-  n_tiles = (g.npad + n_tile - 1) / n_tile;
+  while (kNt[ni] * pl.n_tiles < g.npad) ++ni;
+  pl.n_tiles = (g.npad + kNt[ni] - 1) / kNt[ni];
   const int sms = sm_count();
-  // FSB_CONV_NTILE_MIN: smallest N tile the split may produce (default 32).  Splitting N does not shorten a CTA's main loop
-  // (every tap and channel chunk is still walked); it spreads the weight loads and the epilogue over more SMs.
-  const int nt_min = opt(OPT_CONV_NTILE_MIN) >= 16 ? opt(OPT_CONV_NTILE_MIN) : 32;
-  while (m_tiles * n_tiles < sms && ni > 0 && kNt[ni - 1] >= nt_min) {
-    n_tile = kNt[--ni];
-    n_tiles = (g.npad + n_tile - 1) / n_tile;
+  while (pl.m_tiles * pl.n_tiles < sms && ni > 0 && kNt[ni - 1] >= 32) {
+    --ni;
+    pl.n_tiles = (g.npad + kNt[ni] - 1) / kNt[ni];
   }
-  // A grid of at most one CTA per SM is bound by each CTA's latency, not by L2 -> SM traffic; there the window mode's wait for
-  // a whole window before the first MMA makes it slower (by 7-19 % on the student's 1/16 and 1/32 maps), so it runs only on
-  // larger grids unless FSB_CONV_TC2=1 forces it.  The training convs (BN-train statistics, and the data gradient, whose
+  pl.n_tile = kNt[ni];
+  const int ctas = pl.m_tiles * pl.n_tiles;
+  // Window mode (3x3 stride-1 dilation-1 convs without custom tap tables): the per-tap mode moves every input byte of a tile
+  // from L2 to the SM nine times, and on large maps L2 -> SM bandwidth bounds the kernel (DESIGN.md section 3.3).  A grid of at
+  // most one CTA per SM is bound by each CTA's latency instead, where waiting for a whole window before the first MMA is slower
+  // (by 7-19 % on the student's 1/16 and 1/32 maps).  The training convs (BN-train statistics, and the data gradient, whose
   // caller passes window_ok = false) stay per-tap: with them in window mode the distillation step measured slower.
-  const bool win = strip || (mode == kWindow && ((window_ok && m_tiles * n_tiles > sms && !(d->flags & FSB_CONV_STATS)) ||
-                                                 opt(OPT_CONV_TC2) == 1));
+  // FSB_CONV_TC2=0 forces the per-tap mode and 1 the window mode wherever it can run (for A/B measurements and tests).
+  const int tc2 = opt(OPT_CONV_TC2);
+  const bool win_ok = !cu && d->ksize == 3 && d->stride == 1 && d->dil == 1 && tc2 != 0;
+  pl.win = win_ok && ((window_ok && ctas > sms && !(d->flags & FSB_CONV_STATS)) || tc2 == 1);
   // window mode: 64-channel chunks for every Cin; a ragged last chunk is zero-filled by TMA on both operands (the input map
   // ends at Cin, the weight map at kpad)
-  const int bk = win ? 64 : g.bk;
-  p.k_chunks = (g.kpad + bk - 1) / bk;
-  if (win) {
-    p.win_pitch = p.tw + 2;
-    p.win_rows = p.th + 2;
-    p.win_stride = (p.win_rows * p.win_pitch * 128 + 1023) / 1024 * 1024;
-    p.m_half = 64;
-    p.m_grp = 8;
-    if (strip) {
-      p.win_sbo = 8 * 128;
-      p.win_half = 64;
-    } else if (p.tw == 16) {
-      p.win_sbo = p.win_pitch * 128;
-      p.win_half = 8;
-      p.m_half = 8;
-      p.m_grp = 16;
-    } else {
-      p.win_sbo = p.win_pitch * 128;
-      p.win_half = 8 * p.win_pitch;
+  pl.bk = pl.win ? 64 : g.bk;
+  pl.k_chunks = (g.kpad + pl.bk - 1) / pl.bk;
+  if (pl.win) {
+    pl.win_pitch = pl.tw + 2;
+    pl.win_rows = pl.th + 2;
+    pl.win_stride = (pl.win_rows * pl.win_pitch * 128 + 1023) / 1024 * 1024;
+    pl.win_sbo = pl.win_pitch * 128;
+    pl.win_half = 8 * pl.win_pitch;
+    pl.m_half = 64;
+    pl.m_grp = 8;
+    if (pl.tw == 16) {
+      pl.win_half = 8;
+      pl.m_half = 8;
+      pl.m_grp = 16;
     }
   }
+  // Residency res = the CTAs per SM the launch can use: at most what the instance's registers allow (conv_tc_residency) and at
+  // most what the grid fills (CTAs / SMs, rounded up).  A multi-wave conv is bound by how many CTAs overlap on an SM (DESIGN.md
+  // section 3.3); a grid of 1-2 CTAs per SM gains nothing from a third slot and keeps the deeper ring.  Budget of the windows +
+  // stage ring: one CTA per SM gets (almost) the whole shared memory; otherwise an SM's 227 KB shared by res CTAs, less each
+  // CTA's static shared memory, the 1 KB the driver reserves per CTA and the 1 KB of slack that aligns the ring.
+  const size_t stage_bytes = (pl.win ? 0 : static_cast<size_t>(kTileM) * pl.bk * 2) + static_cast<size_t>(pl.n_tile) * pl.bk * 2;
+  const int grid_res = (ctas + sms - 1) / sms;
+  pl.res = grid_res < conv_tc_residency(pl.n_tile) ? grid_res : conv_tc_residency(pl.n_tile);
+  const size_t budget = pl.res <= 1 ? 200 * 1024 : 227 * 1024 / pl.res - conv_tc_static_smem(pl.n_tile) - 2 * 1024;
+  const size_t win_bytes = pl.win ? 2 * static_cast<size_t>(pl.win_stride) : 0;  // two input windows ahead of the weight ring
+  pl.stages = static_cast<int>((budget - win_bytes) / stage_bytes);
+  if (pl.stages < 2) pl.stages = 2;
+  if (pl.stages > kMaxStages) pl.stages = kMaxStages;
+  if (pl.stages > pl.taps * pl.k_chunks) pl.stages = pl.taps * pl.k_chunks;
+  // The ring and windows, or the epilogue's reuse of them, and at least the whole budget: allocated in full, no more than res
+  // CTAs share an SM.  The registers of a 160-thread instance leave room for more (up to 4 CTAs per SM at 96 registers), and
+  // left that way the grids of at most one or two CTAs per SM measured slower than with 256-thread CTAs (DESIGN.md section 3.3).
+  size_t smem = win_bytes + stage_bytes * pl.stages;
+  if (smem < conv_tc_epilogue_bytes(pl.n_tile)) smem = conv_tc_epilogue_bytes(pl.n_tile);
+  if (smem < budget) smem = budget;
+  pl.smem = smem + 1024;  // + the slack that aligns the ring to 1024 B
+  return pl;
+}
+
+// The kernel instance a plan runs: (BK, NT, WIN) and, for FSB_CONV_Y_UP2, conv_tc_up2_kernel.  The launch and the occupancy
+// query both select it here; entry is the pointer of the two that the plan runs, its dynamic shared-memory limit raised.
+struct ConvTcInstance {
+  void (*plain)(ConvTcParams);
+  void (*up2)(ConvTcUp2Params);
+  const void* entry;
+};
+
+template <int BK, bool WIN>
+static ConvTcInstance conv_tc_instance_nt(int n_tile) {
+  switch (n_tile) {
+    case 16: return {conv_tc_kernel<BK, 16, WIN>, conv_tc_up2_kernel<BK, 16, WIN>, nullptr};
+    case 32: return {conv_tc_kernel<BK, 32, WIN>, conv_tc_up2_kernel<BK, 32, WIN>, nullptr};
+    case 48: return {conv_tc_kernel<BK, 48, WIN>, conv_tc_up2_kernel<BK, 48, WIN>, nullptr};
+    case 64: return {conv_tc_kernel<BK, 64, WIN>, conv_tc_up2_kernel<BK, 64, WIN>, nullptr};
+    case 96: return {conv_tc_kernel<BK, 96, WIN>, conv_tc_up2_kernel<BK, 96, WIN>, nullptr};
+    default: return {conv_tc_kernel<BK, 128, WIN>, conv_tc_up2_kernel<BK, 128, WIN>, nullptr};
+  }
+}
+
+static int conv_tc_instance(const ConvPlan& pl, ConvTcInstance* k) {
+  if (pl.win) *k = conv_tc_instance_nt<64, true>(pl.n_tile);
+  else if (pl.bk == 64) *k = conv_tc_instance_nt<64, false>(pl.n_tile);
+  else *k = conv_tc_instance_nt<32, false>(pl.n_tile);
+  k->entry = pl.up2 ? reinterpret_cast<const void*>(k->up2) : reinterpret_cast<const void*>(k->plain);
+  return ensure_dyn_smem(k->entry, 220 * 1024, "cudaFuncSetAttribute(conv_tc)");
+}
+
+int conv_tc_occupancy(const ConvPlan& plan) {
+  ConvTcInstance k;
+  if (int rc = conv_tc_instance(plan, &k)) return rc;
+  int ctas = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, k.entry, kThreads, plan.smem);
+  return e == cudaSuccess ? ctas : set_cuda_error(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_tc)");
+}
+
+int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale,
+                   const float* shift, void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu) {
+  if (plan.rc) return plan.rc;
+  if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(wpacked) & 15))
+    return set_error(FSB_ERR_INVALID, "conv_tc: x / wpacked must be 16-byte aligned");
+  const ConvGeom g = conv_geom(d);
+  ConvTcUp2Params q;
+  memset(&q, 0, sizeof(q));
+  ConvTcParams& p = q.p;
+  p.taps = plan.taps;
+  p.Ho = plan.Ho;
+  p.Wo = plan.Wo;
+  p.tw = plan.tw;
+  p.th = plan.th;
+  p.tiles_w = plan.tiles_w;
+  p.tiles_h = plan.tiles_h;
+  for (int i = 0; i < 9; ++i) p.tap_widx[i] = i;
+  p.Cout = d->Cout;
+  p.k_chunks = plan.k_chunks;
+  p.win_pitch = plan.win_pitch;
+  p.win_rows = plan.win_rows;
+  p.win_sbo = plan.win_sbo;
+  p.win_half = plan.win_half;
+  p.win_stride = plan.win_stride;
+  p.m_half = plan.m_half;
+  p.m_grp = plan.m_grp;
+  p.stages = plan.stages;
   p.y_cstride = d->y_cstride;
   p.flags = d->flags;
   p.scale = scale;
@@ -630,51 +662,14 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   p.stats_off = d->stats_off;
   if ((d->flags & FSB_CONV_STATS) && stats && (d->stats_off < 0 || d->stats_off + d->Cout > p.stats_C))
     return set_error(FSB_ERR_INVALID, "conv_tc: stats_off + Cout exceeds stats_C");
-
-  const size_t stage_bytes = (win ? 0 : static_cast<size_t>(kTileM) * bk * 2) + static_cast<size_t>(n_tile) * bk * 2;
-  const int k_iters = p.taps * p.k_chunks;
-  // Residency res = the CTAs per SM the launch can use: at most what the instance's registers allow (conv_tc_residency) and at
-  // most what the grid fills (CTAs / SMs, rounded up).  A multi-wave conv is bound by how many CTAs overlap on an SM (DESIGN.md
-  // section 3.3); a grid of 1-2 CTAs per SM gains nothing from a third slot and keeps the deeper ring.  Budget of the windows +
-  // stage ring: one CTA per SM (and the row strip, whose windows alone take 100 KB) gets (almost) the whole shared memory;
-  // otherwise an SM's 227 KB shared by res CTAs, less each CTA's static shared memory, the 1 KB the driver reserves per CTA and
-  // the 1 KB of slack that aligns the ring.
-  const int grid_res = (m_tiles * n_tiles + sms - 1) / sms;
-  const int res = strip ? 1 : (grid_res < conv_tc_residency(n_tile) ? grid_res : conv_tc_residency(n_tile));
-  const size_t smem_budget = res <= 1 ? 200 * 1024 : 227 * 1024 / res - conv_tc_static_smem(n_tile) - 2 * 1024;
-  const size_t win_bytes = win ? 2 * static_cast<size_t>(p.win_stride) : 0;   // two input windows ahead of the weight ring
-  int stages = static_cast<int>((smem_budget - win_bytes) / stage_bytes);
-  if (stages < 2) stages = 2;
-  if (stages > kMaxStages) stages = kMaxStages;
-  if (stages > k_iters) stages = k_iters;
-  p.stages = stages;
-  const size_t epi_bytes = n_tile == 16 ? conv_tc_epilogue_bytes<16>() : n_tile == 32 ? conv_tc_epilogue_bytes<32>()
-                           : n_tile == 48 ? conv_tc_epilogue_bytes<48>() : n_tile == 64 ? conv_tc_epilogue_bytes<64>()
-                           : n_tile == 96 ? conv_tc_epilogue_bytes<96>() : conv_tc_epilogue_bytes<128>();
-  size_t smem_bytes = (win_bytes + stage_bytes * stages > epi_bytes ? win_bytes + stage_bytes * stages : epi_bytes) + 1024;
-  // Allocate the whole budget, so that no more than res CTAs share an SM.  The registers of a 160-thread instance leave room for
-  // more (up to 4 CTAs per SM at 96 registers), and left that way the grids of at most one or two CTAs per SM measured slower
-  // than with 256-thread CTAs (DESIGN.md section 3.3).
-  if (smem_bytes < smem_budget + 1024) smem_bytes = smem_budget + 1024;
-  const dim3 grid(static_cast<unsigned>(m_tiles), static_cast<unsigned>(n_tiles));
-  auto run = [&]() {
-    if (win) return conv_tc_run_nt<64, true>(n_tile, grid, smem_bytes, stream, q, residency);
-    if (g.bk == 64) return conv_tc_run_nt<64, false>(n_tile, grid, smem_bytes, stream, q, residency);
-    return conv_tc_run_nt<32, false>(n_tile, grid, smem_bytes, stream, q, residency);
-  };
-  if (residency) {  // the query needs only the instance and its shared memory, not the tensor maps
-    q.y_reps = (d->flags & FSB_CONV_Y_UP2) ? 4 : 1;
-    return run();
-  }
   // ---- TMA-store epilogue: fp16 output whose pixels start on 16 B and whose channel count is a multiple of 8 ----
   // FSB_CONV_Y_UP2: y is the 2Ho x 2Wo map and every output pixel goes to its 2x2 block (nearest x2 folded into the store):
   // four lattice maps, one per (row, column) parity, each with the pixel steps of the full map doubled; the epilogue stores
   // every staged slab to each of them.
-  const bool up2 = (d->flags & FSB_CONV_Y_UP2) != 0;
   p.tma_store = 0;
   q.y_reps = 1;
   if (!(d->flags & (FSB_CONV_OUT_F32 | FSB_CONV_STATS)) && d->Cout % 8 == 0 && d->y_cstride % 8 == 0 && (reinterpret_cast<uintptr_t>(y) & 15) == 0 &&
-      n_tile % 8 == 0 && (cu || up2 || opt(OPT_NO_TMA_STORE) <= 0)) {
+      plan.n_tile % 8 == 0) {
     const uint64_t ycs = static_cast<uint64_t>(d->y_cstride) * 2;
     uint64_t dims[4] = {static_cast<uint64_t>(d->Cout), static_cast<uint64_t>(d->Wo), static_cast<uint64_t>(d->Ho),
                         static_cast<uint64_t>(d->N)};
@@ -685,7 +680,7 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
       for (int i = 0; i < 4; ++i) dims[i] = cu->y_dims[i];
       for (int i = 0; i < 3; ++i) str[i] = cu->y_strides[i];
     }
-    if (up2) {
+    if (plan.up2) {
       q.y_reps = 4;
       const uint64_t row = ycs * 2 * d->Wo;  // one row of the 2Ho x 2Wo map
       str[0] = 2 * ycs;
@@ -694,35 +689,35 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
       for (int l = 0; l < 4; ++l) ybase[l] = static_cast<const uint8_t*>(y) + (l >> 1) * row + (l & 1) * ycs;
     }
     const uint32_t box64[4] = {64u, static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
-    p.tail_w = n_tile % 64;
+    p.tail_w = plan.n_tile % 64;
     const uint32_t boxt[4] = {static_cast<uint32_t>(p.tail_w), static_cast<uint32_t>(p.tw), static_cast<uint32_t>(p.th), 1u};
     for (int l = 0; l < q.y_reps; ++l) {
       CUtensorMap* maps = l == 0 ? p.tmap_y : q.tmap_up + 2 * (l - 1);
       int rc = 0;
-      if (n_tile >= 64) rc = encode_tiled(&maps[0], ybase[l], 4, dims, str, box64, 128);
+      if (plan.n_tile >= 64) rc = encode_tiled(&maps[0], ybase[l], 4, dims, str, box64, 128);
       if (!rc && p.tail_w) rc = encode_tiled(&maps[1], ybase[l], 4, dims, str, boxt, 0);
       if (rc) return rc;
-      if (n_tile < 64) maps[0] = maps[1];
+      if (plan.n_tile < 64) maps[0] = maps[1];
     }
     p.tma_store = 1;
   }
   if (cu && !p.tma_store) return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: custom output lattice needs the TMA-store epilogue");
-  if (up2 && !p.tma_store)
+  if (plan.up2 && !p.tma_store)
     return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_Y_UP2 needs the TMA-store epilogue (fp16 output, Cout and y_cstride "
                                           "multiples of 8, 16-byte aligned y)");
 
   // ---- A tensor maps ----
   const __half* xb = static_cast<const __half*>(x);
   const uint64_t cs = static_cast<uint64_t>(d->x_cstride) * 2;  // bytes per pixel step
-  const uint32_t boxA[4] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(win ? p.win_pitch : p.tw),
-                            static_cast<uint32_t>(win ? p.win_rows : p.th), 1u};
+  const uint32_t boxA[4] = {static_cast<uint32_t>(plan.bk), static_cast<uint32_t>(plan.win ? p.win_pitch : p.tw),
+                            static_cast<uint32_t>(plan.win ? p.win_rows : p.th), 1u};
   if (d->stride == 1) {
     const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
                               static_cast<uint64_t>(d->N)};
     // FSB_CONV_X_DOWN2: x is the 2H x 2W map and the conv reads its even rows and columns (nearest /2 folded into the load)
     const bool down2 = (d->flags & FSB_CONV_X_DOWN2) != 0;
     const uint64_t str[3] = {down2 ? 2 * cs : cs, down2 ? 4 * cs * d->W : cs * d->W, down2 ? 4 * cs * d->W * d->H : cs * d->W * d->H};
-    int rc = encode_tiled(&p.tmap_a[0], xb, 4, dims, str, boxA, bk * 2);
+    int rc = encode_tiled(&p.tmap_a[0], xb, 4, dims, str, boxA, plan.bk * 2);
     if (rc) return rc;
     for (int r = 0; r < d->ksize; ++r)
       for (int s = 0; s < d->ksize; ++s) {
@@ -770,11 +765,16 @@ int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, c
   {
     const uint64_t dims[3] = {static_cast<uint64_t>(g.kpad), static_cast<uint64_t>(g.npad), static_cast<uint64_t>(g.taps)};
     const uint64_t str[2] = {static_cast<uint64_t>(g.kpad) * 2, static_cast<uint64_t>(g.kpad) * g.npad * 2};
-    const uint32_t boxB[3] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(n_tile), 1u};
-    int rc = encode_tiled(&p.tmap_b, wpacked, 3, dims, str, boxB, bk * 2);
+    const uint32_t boxB[3] = {static_cast<uint32_t>(plan.bk), static_cast<uint32_t>(plan.n_tile), 1u};
+    int rc = encode_tiled(&p.tmap_b, wpacked, 3, dims, str, boxB, plan.bk * 2);
     if (rc) return rc;
   }
-  return run();
+  ConvTcInstance k;
+  if (int rc = conv_tc_instance(plan, &k)) return rc;
+  const dim3 grid(static_cast<unsigned>(plan.m_tiles), static_cast<unsigned>(plan.n_tiles));
+  const cudaError_t e = plan.up2 ? launch_kernel(k.up2, grid, dim3(kThreads), plan.smem, stream, q)
+                                 : launch_kernel(k.plain, grid, dim3(kThreads), plan.smem, stream, q.p);
+  return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
 }
 
 }  // namespace fsb

@@ -18,6 +18,10 @@ typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_
                                     const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                     CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 PFN_encodeTiled get_encode_tiled();
+// cuTensorMapEncodeTiled of an fp16 tensor (rank <= 5, dims / strides innermost first, strides in bytes) with a 128/64/32-byte or
+// no swizzle; errors land in fsb_last_error_string
+int encode_tiled(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
+                 const uint32_t* box, int swizzle_bytes);
 
 // derived geometry shared by the packer and the kernels
 struct ConvGeom {
@@ -30,28 +34,17 @@ ConvGeom conv_geom(const fsb_conv_desc* d);
 
 bool pdl_enabled();
 int sm_count();
+int stat_rows(int64_t pixels);  // partial statistic rows of the CUDA-core kernels (bn.cu)
 
 // Tuning / validation switches.  Read from the environment ONCE (first use) and settable through fsb_set_option(); never a
-// getenv() on the launch path.  -1 = unset.  The switches marked "no effect" selected conv kernel variants that this sm_90a
-// library does not have; their names stay accepted so that existing settings keep working.
+// getenv() on the launch path.  -1 = unset.
 enum Opt {
-  OPT_CONV_TC2 = 0,      // FSB_CONV_TC2: mode of conv_tc for 3x3 stride-1 convs: 0 = per-tap, 1 = window, 2 = row strip
+  OPT_CONV_TC2 = 0,      // FSB_CONV_TC2: mode of conv_tc for 3x3 stride-1 convs: 0 = per-tap, 1 = window
                          // (default: window on inference convs with more CTAs than SMs, else per-tap)
-  OPT_TC2_R,             // FSB_TC2_R: no effect
-  OPT_TC2_ASTAGES,       // FSB_TC2_ASTAGES: no effect
-  OPT_NO_TMA_STORE,      // FSB_NO_TMA_STORE
   OPT_DGRAD_S2_DIRECT,   // FSB_DGRAD_S2_DIRECT
   OPT_WGRAD_TC,          // FSB_WGRAD_TC: 0 = CUDA-core weight gradient
-  OPT_CONV_PERSIST,      // FSB_CONV_PERSIST: no effect
-  OPT_PERSIST_OCC,       // FSB_PERSIST_OCC: no effect
-  OPT_PERSIST_STAGES,    // FSB_PERSIST_STAGES: no effect
   OPT_UPSAMPLE_V2,       // FSB_UPSAMPLE_V2
   OPT_DETERMINISTIC,     // FSB_DETERMINISTIC: 1 = weight gradients without split-K atomics (bit-reproducible steps)
-  OPT_CONV_TC3,          // FSB_CONV_TC3: no effect
-  OPT_CONV_TC4,          // FSB_CONV_TC4: no effect
-  OPT_CONV_TC5,          // FSB_CONV_TC5: no effect
-  OPT_CONV_KSPLIT,       // FSB_CONV_KSPLIT: no effect
-  OPT_CONV_NTILE_MIN,    // FSB_CONV_NTILE_MIN: lower bound of the output-channel tile when conv_tc splits N to occupy more SMs (default 32)
   OPT_COUNT
 };
 int opt(Opt o);
@@ -100,12 +93,32 @@ struct ConvTcCustom {
   uint64_t y_strides[3];  // bytes: lattice step in W, in H, image
 };
 int conv_tc_supported(const fsb_conv_desc* d);
-bool conv_tc_strip(const fsb_conv_desc* d);  // conv_tc runs d in row-strip mode
-// window_ok = false keeps a 3x3 stride-1 problem on the per-tap mode unless FSB_CONV_TC2 forces the window mode;
-// residency != nullptr launches nothing and stores the CTAs per SM of the instance and shared memory the call would launch with
-int conv_tc_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
-                   void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr, bool window_ok = true,
-                   int* residency = nullptr);
+
+// Every decision of one conv launch, taken from the descriptor alone (conv_plan reads no data pointer and makes no CUDA call
+// but sm_count()).  The launch, the statistics-row, kernel-id and residency queries and the fused BN-train forward all read it.
+struct ConvPlan {
+  int rc;                  // FSB_OK, or the error a launch of this descriptor returns; the fields below are filled either way
+  bool direct;             // CUDA-core direct kernel (FSB_CONV_FORCE_DIRECT, or a problem conv_tc cannot run); the rest is conv_tc's
+  int stat_rows;           // partial statistic rows written with FSB_CONV_STATS: stat_rows(N * Ho * Wo) direct, m_tiles on conv_tc
+  bool win;                // window mode (one halo window per 64-channel chunk) instead of per-tap
+  bool up2;                // FSB_CONV_Y_UP2: the instance that also stores the other three 2x2 lattices
+  int taps, Ho, Wo;        // taps and output extent of the tiling (a custom lattice's own)
+  int tw, th;              // 128-pixel tile: 16 x 8, or 8 x 16 when Wo < 16
+  int tiles_w, tiles_h, m_tiles;
+  int n_tile, n_tiles;     // output channels per CTA (the instance's NT) and CTAs along N
+  int bk, k_chunks;        // channels per K chunk (the instance's BK) and chunks per tap
+  int win_pitch, win_rows, win_sbo, win_half, win_stride, m_half, m_grp;  // window geometry, see ConvTcParams (conv_tc.cu)
+  int res, stages;         // CTAs per SM the shared memory is sized for, depth of the stage ring
+  size_t smem;             // dynamic shared memory of the launch
+};
+// window_ok = false keeps a 3x3 stride-1 problem on the per-tap mode unless FSB_CONV_TC2 forces the window mode; cu (custom tap
+// tables) always runs per-tap
+ConvPlan conv_plan(const fsb_conv_desc* d, const ConvTcCustom* cu = nullptr, bool window_ok = true);
+// launch conv_tc as planned (plan = conv_plan(d, cu, ...), not direct)
+int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale,
+                   const float* shift, void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr);
+// CTAs per SM of the planned conv_tc launch, from the CUDA occupancy calculator; launches nothing
+int conv_tc_occupancy(const ConvPlan& plan);
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride);
 int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
                          float gscale, cudaStream_t stream);

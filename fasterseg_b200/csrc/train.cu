@@ -207,7 +207,6 @@ static inline unsigned grid_for(int64_t total, int threads) {
   return static_cast<unsigned>(b);
 }
 
-int stat_rows(int64_t pixels);
 int rowsum_launch(int L, const float* rows, int P, int stride, float* out, cudaStream_t stream);
 
 // sums: (1 + stat_rows(pixels)) rows of 2*C floats; the partial rows land in rows 1.., their fixed-order total in row 0
@@ -378,7 +377,7 @@ int conv_dgrad_launch(const fsb_conv_desc* d, const void* dy, int dcs, const voi
                       int64_t si, void* dx, int xcs, cudaStream_t stream) {
   if (d->stride == 1 && d->off_h == 0 && d->off_w == 0 && wpacked_t && !(d->flags & FSB_CONV_FORCE_DIRECT)) {
     fsb_conv_desc t = dgrad_as_fwd_desc(d, dcs, xcs);
-    if (conv_tc_supported(&t)) return conv_tc_launch(&t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream, nullptr, false);
+    if (conv_tc_supported(&t)) return conv_tc_launch(conv_plan(&t, nullptr, false), &t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream);
   }
   // stride 2: the input pixels of each (row, column) parity receive contributions from a fixed subset of filter taps; each
   // parity plane is a stride-1 implicit GEMM over dy with that tap subset, written to the plane through a strided tensor map
@@ -429,7 +428,7 @@ int conv_dgrad_launch(const fsb_conv_desc* d, const void* dy, int dcs, const voi
     if (conv_tc_supported(&t)) {
       for (int i = 0; i < 4; ++i) {
         if (!live[i]) continue;
-        int rc = conv_tc_launch(&t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream, &planes[i]);
+        int rc = conv_tc_launch(conv_plan(&t, &planes[i]), &t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream, &planes[i]);
         if (rc) return rc;
       }
       return FSB_OK;

@@ -15,8 +15,6 @@ int bn_bwd_apply_launch(int64_t, int, const void*, int, const void*, int, const 
                         const float*, const float*, double, int, void*, int, float*, float*, float, cudaStream_t, int,
                         const fsb_bn_sel*, const int*, int, const float*);
 int rowsum_launch(int, const float*, int, int, float*, cudaStream_t);
-int conv_tc_m_tiles(const fsb_conv_desc*);
-int stat_rows(int64_t);
 int conv_dgrad_launch(const fsb_conv_desc*, const void*, int, const void*, const float*, int64_t, int64_t, void*, int, cudaStream_t);
 int conv_wgrad_launch(const fsb_conv_desc*, const void*, const void*, int, float*, int64_t, int64_t, int, float, cudaStream_t);
 int dp_world();                                        // dp.cu: 1 unless fsb_dp_init created a communicator
@@ -62,11 +60,11 @@ int fsb_conv_bn_act_train_fwd(const fsb_conv_desc* d, const void* x, const void*
   c.stats_C = 0;
   c.stats_off = 0;
   float* rows = vec + 6 * C;
-  const bool direct = (c.flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(&c);
+  const ConvPlan plan = conv_plan(&c);
   const int64_t pixels = static_cast<int64_t>(d->N) * d->Ho * d->Wo;
-  int R = direct ? stat_rows(pixels) : conv_tc_m_tiles(&c);
-  int rc = direct ? conv_direct_launch(&c, x, wpacked, nullptr, nullptr, raw_f32, rows, st)
-                  : conv_tc_launch(&c, x, wpacked, nullptr, nullptr, raw_f32, rows, st);
+  int R = plan.stat_rows;
+  int rc = plan.direct ? conv_direct_launch(&c, x, wpacked, nullptr, nullptr, raw_f32, rows, st)
+                       : conv_tc_launch(plan, &c, x, wpacked, nullptr, nullptr, raw_f32, rows, st);
   if (rc) return rc;
   const int world = dp_world();
   const float* stats = rows;

@@ -151,9 +151,6 @@ conv_wgrad_tc_kernel(const __grid_constant__ WgradTcParams p) {
   __syncthreads();
 }
 
-int encode_tiled_generic(CUtensorMap* map, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                         const uint32_t* box, int swizzle_bytes);
-
 static inline int floordiv2(int a) { return (a >= 0) ? a / 2 : -((-a + 1) / 2); }
 
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride) {
@@ -210,7 +207,7 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
     const uint64_t dims[4] = {static_cast<uint64_t>(d->Cout), static_cast<uint64_t>(d->Wo), static_cast<uint64_t>(d->Ho),
                               static_cast<uint64_t>(d->N)};
     const uint64_t str[3] = {cs, cs * d->Wo, cs * d->Wo * d->Ho};
-    int rc = encode_tiled_generic(&p.tmap_dy, dy, 4, dims, str, box, 128);
+    int rc = encode_tiled(&p.tmap_dy, dy, 4, dims, str, box, 128);
     if (rc) return rc;
   }
   const __half* xb = static_cast<const __half*>(x);
@@ -219,7 +216,7 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
     const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(d->W), static_cast<uint64_t>(d->H),
                               static_cast<uint64_t>(d->N)};
     const uint64_t str[3] = {cs, cs * d->W, cs * d->W * d->H};
-    int rc = encode_tiled_generic(&p.tmap_x[0], xb, 4, dims, str, box, 128);
+    int rc = encode_tiled(&p.tmap_x[0], xb, 4, dims, str, box, 128);
     if (rc) return rc;
     for (int r = 0; r < d->ksize; ++r)
       for (int s = 0; s < d->ksize; ++s) {
@@ -248,8 +245,8 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
         const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(Wp), static_cast<uint64_t>(Hp),
                                   static_cast<uint64_t>(d->N)};
         const uint64_t str[3] = {2 * cs, 2 * cs * d->W, cs * d->W * d->H};
-        int rc = encode_tiled_generic(&p.tmap_x[ph * 2 + pw], xb + (static_cast<size_t>(ph) * d->W + pw) * d->x_cstride, 4, dims,
-                                      str, box, 128);
+        int rc = encode_tiled(&p.tmap_x[ph * 2 + pw], xb + (static_cast<size_t>(ph) * d->W + pw) * d->x_cstride, 4, dims,
+                              str, box, 128);
         if (rc) return rc;
       }
   }

@@ -108,16 +108,14 @@ int fsb_device_info(int* sm_count, int* cc_major, int* cc_minor);
 /* Programmatic dependent launch between consecutive kernels of this library (default on; env FSB_PDL=0 disables).
  * With it a kernel's prologue (barrier init, descriptor prefetch) overlaps its predecessor's tail. */
 int fsb_set_pdl(int enabled);
-/* Tuning / validation switches, named like their environment variables (FSB_CONV_TC2: row-strip mode of the conv kernel,
- * FSB_NO_TMA_STORE, FSB_DGRAD_S2_DIRECT, FSB_WGRAD_TC, FSB_UPSAMPLE_V2, FSB_DETERMINISTIC, FSB_CONV_NTILE_MIN).  The names of
- * switches of earlier kernel variants (FSB_TC2_R, FSB_TC2_ASTAGES, FSB_CONV_TC3..5, FSB_CONV_PERSIST, FSB_PERSIST_OCC,
- * FSB_PERSIST_STAGES, FSB_CONV_KSPLIT) are still accepted and have no effect.  The environment is read once at first use;
- * value -1 = unset. */
+/* Tuning / validation switches, named like their environment variables (FSB_CONV_TC2: mode of the conv kernel for 3x3
+ * stride-1 convs, 0 = per-tap, 1 = window, unset = chosen per problem; FSB_DGRAD_S2_DIRECT, FSB_WGRAD_TC, FSB_UPSAMPLE_V2,
+ * FSB_DETERMINISTIC).  The environment is read once at first use; value -1 = unset.  FSB_ERR_INVALID for any other name. */
 int fsb_set_option(const char* name, int value);
 int fsb_get_option(const char* name);
 
-/* Developer aid: when set (device buffer of 128 uint64), the row-strip conv kernel records %globaltimer stamps of its
- * pipeline phases for the first and last CTA.  NULL disables (default). */
+/* Developer aid: registers a device buffer (128 uint64) for in-kernel timelines of experimental kernels.  No kernel of this
+ * build writes it.  NULL disables (default). */
 int fsb_debug_set_buffer(void* dev_u64x128);
 
 /* --- weights -------------------------------------------------------------------------------- */
@@ -143,9 +141,8 @@ int fsb_bn_fold(int C, const float* gamma, const float* beta, const float* mean,
 int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
                  void* y, float* stats, void* stream);
 /* which kernel fsb_conv_fwd dispatches for `d`: 0 = CUDA-core direct, 1 = the wgmma kernel conv_tc on 16x8 / 8x16 pixel tiles
- * (per-tap mode, or window mode: one halo window of the input per 64-channel chunk, taps as descriptor offsets), 2 = conv_tc
- * in row-strip mode (the window mode on 128x1 tiles, FSB_CONV_TC2=2); negative = invalid descriptor.  y and with_stats are
- * accepted for compatibility and do not change the choice. */
+ * (per-tap mode, or window mode: one halo window of the input per 64-channel chunk, taps as descriptor offsets); negative =
+ * invalid descriptor.  y and with_stats are accepted for compatibility and do not change the choice. */
 int fsb_conv_kernel_id(const fsb_conv_desc* d, const void* y, int with_stats);
 /* number of partial statistic rows fsb_conv_fwd writes for `d` with FSB_CONV_STATS (depends on the kernel it dispatches):
  * stats must hold rows * 2 * SC floats; every row's entries of this conv's channels are written (no zeroing needed). */

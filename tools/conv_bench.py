@@ -1,9 +1,9 @@
 #!/usr/bin/env python
 """Per-layer micro-benchmark of the conv / resize kernels on the student's layer shapes (1x3x1024x2048 frame).
 Prints us/launch, achieved TFLOP/s and algorithmic GB/s per layer; `--only i` restricts to one layer.
-`--compare`: on every layer time conv_tc's per-tap mode (FSB_CONV_TC2=0), its default (window mode on 3x3 stride-1 convs) and,
-where it applies, the row strip (FSB_CONV_TC2=2), alternating them `--rounds` times in this process; print the median us of
-each and the L2 -> SM bytes each mode moves (TMA boxes of input and weights, from conv_tc_launch's tiling rule)."""
+`--compare`: on every layer time conv_tc's per-tap mode (FSB_CONV_TC2=0) and, on 3x3 stride-1 convs, its window mode
+(FSB_CONV_TC2=1), alternating them `--rounds` times in this process; print the median us of each and the L2 -> SM bytes each
+mode moves (TMA boxes of input and weights, from conv_plan's tiling rule)."""
 import argparse
 import os
 import sys
@@ -49,13 +49,13 @@ SMS = 132  # H100 SXM
 
 
 def l2_to_sm_mb(ci, co, k, s, h, w, mode):
-    """(MB of TMA boxes one launch loads into shared memory in `mode` ("per-tap", "window" or "strip"), CTAs), following
-    conv_tc_launch: 16 x 8 tiles (8 x 16 when Wo < 16, 128 x 1 for the strip), N tile of <= 128 channels split while the grid has
-    fewer CTAs than SMs; per-tap: one input box of 128 px x BK and one weight box per (tap, chunk); window / strip: one
-    (th + 2) x (tw + 2) px x 64-channel window per chunk and one weight box per (chunk, tap)."""
+    """(MB of TMA boxes one launch loads into shared memory in `mode` ("per-tap" or "window"), CTAs), following
+    conv_plan: 16 x 8 tiles (8 x 16 when Wo < 16), N tile of <= 128 channels split while the grid has fewer CTAs than SMs;
+    per-tap: one input box of 128 px x BK and one weight box per (tap, chunk); window: one (th + 2) x (tw + 2) px x 64-channel
+    window per chunk and one weight box per (chunk, tap)."""
     pad = 1 if k == 3 else 0
     ho, wo = (h + 2 * pad - k) // s + 1, (w + 2 * pad - k) // s + 1
-    tw = 128 if mode == "strip" else (16 if wo >= 16 else 8)
+    tw = 16 if wo >= 16 else 8
     th = 128 // tw
     m_tiles = -(-wo // tw) * -(-ho // th)
     npad = -(-co // 16) * 16
@@ -124,10 +124,8 @@ def main():
             return st.elapsed_time(en) * 1000 / args.reps
 
         if args.compare:
-            # FSB_CONV_TC2: 0 = per-tap, 1 = window, 2 = row strip; unset (the default) = window on grids of more CTAs than SMs
-            modes = {"per-tap": 0, "window": 1, "strip": 2} if k == 3 and s == 1 else {"per-tap": 0}
-            if ci % 64 != 0:
-                modes.pop("strip", None)
+            # FSB_CONV_TC2: 0 = per-tap, 1 = window; unset (the default) = window on grids of more CTAs than SMs
+            modes = {"per-tap": 0, "window": 1} if k == 3 and s == 1 else {"per-tap": 0}
             graphs = {}
             for label, v in modes.items():
                 _lib.set_option("FSB_CONV_TC2", v)
