@@ -17,6 +17,7 @@ FSB_ACT_IN_F32 = 32
 FSB_CONV_X_DOWN2 = 64
 FSB_CONV_Y_UP2 = 128
 ABI_VERSION = 2
+FSB_ERR_UNSUPPORTED = -3
 
 
 class FsbError(RuntimeError):
@@ -57,6 +58,7 @@ _SIGS = {
     "fsb_conv_fwd": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _P]),
     "fsb_stem_conv_nchw": (C.c_int, [C.c_int] * 4 + [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_uint32, _P]),
     "fsb_stem_conv_u8hwc": (C.c_int, [C.c_int] * 4 + [_P, _P, _P, _P, _P, _P, C.c_int, C.c_uint32, _P]),
+    "fsb_stem_fused": (C.c_int, [C.c_int] * 4 + [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
     "fsb_confusion_matrix": (C.c_int, [C.c_int64, _P, _P, C.c_int, C.c_int, _P, _P]),
     "fsb_bilinear_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, C.c_uint32, _P]),
     "fsb_upsample_logits_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),

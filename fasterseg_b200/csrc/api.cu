@@ -97,6 +97,8 @@ int stem_conv_nchw_launch(int, int, int, int, const void*, int, const float*, co
                           cudaStream_t);
 int stem_conv_u8hwc_launch(int, int, int, int, const uint8_t*, const void*, const float*, const float*, const float*, void*, int, uint32_t,
                            cudaStream_t);
+int stem_fused_launch(int, int, int, int, const void*, const void*, int, const float*, const float*, const float*, int, const void*,
+                      const float*, const float*, void*, int, cudaStream_t);
 int confusion_launch(int64_t, const uint8_t*, const void*, int, int, long long*, cudaStream_t);
 int bilinear_launch(int, int, int, int, int, int, const void*, int, void*, int, uint32_t, cudaStream_t);
 int upsample_logits_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
@@ -314,6 +316,15 @@ int fsb_stem_conv_u8hwc(int N, int H, int W, int Cout, const uint8_t* x, const v
   if (N <= 0 || H <= 0 || W <= 0 || Cout <= 0 || !x || !lut_f16 || !w || !y || y_cstride < Cout)
     return set_error(FSB_ERR_INVALID, "stem_conv_u8hwc: bad argument");
   return stem_conv_u8hwc_launch(N, H, W, Cout, x, lut_f16, w, scale, shift, y, y_cstride, flags, static_cast<cudaStream_t>(stream));
+}
+int fsb_stem_fused(int N, int H, int W, int in_kind, const void* x, const void* lut_f16, int C0, const float* w0, const float* scale0,
+                   const float* shift0, int C1, const void* w1_packed, const float* scale1, const float* shift1, void* y, int y_cstride,
+                   void* stream) {
+  if (N <= 0 || H <= 0 || W <= 0 || in_kind < 0 || in_kind > 2 || !x || (in_kind == 2 && !lut_f16) || !w0 || !scale0 || !shift0 ||
+      !w1_packed || !scale1 || !shift1 || !y || C1 <= 0 || y_cstride < C1)
+    return set_error(FSB_ERR_INVALID, "stem_fused: bad argument");
+  return stem_fused_launch(N, H, W, in_kind, x, lut_f16, C0, w0, scale0, shift0, C1, w1_packed, scale1, shift1, y, y_cstride,
+                           static_cast<cudaStream_t>(stream));
 }
 int fsb_confusion_matrix(int64_t n, const uint8_t* pred, const void* gt, int gt_bytes, int n_cl, long long* out, void* stream) {
   if (n <= 0 || !pred || !gt || !out) return set_error(FSB_ERR_INVALID, "confusion_matrix: bad argument");

@@ -238,6 +238,35 @@ def stem_conv_u8hwc(x_u8, lut, w, scale, shift, relu=True, out=None):
     return out
 
 
+def stem_fused(x, lut, w0, scale0, shift0, w1_packed, C1, scale1, shift1, out=None):
+    """relu(BN(conv1(relu(BN(stem0(x)))))) in one kernel: the RGB stem (w0, fp32 OIHW [C0, 3, 3, 3]) and the 3x3 stride-2 conv1 of
+    stem.1 (w1_packed: pack_conv_weight of its [C1, C0, 3, 3] weight), without the 1/2-resolution map.  x: NCHW fp32 / fp16, or the
+    uint8 HWC view of stem_conv_u8hwc with its `lut`.  Returns `out` (NHWC fp16, 1/4 resolution), or None when the library has no
+    fused kernel for these widths (FSB_ERR_UNSUPPORTED): the caller then runs stem_conv_* and conv_fwd."""
+    assert x.dim() == 4 and x.shape[1] == 3 and _on_device(x)
+    N, _, H, W = x.shape
+    if x.dtype == torch.uint8:
+        assert x.stride() == (H * W * 3, 1, W * 3, 3), "expected the permute(0, 3, 1, 2) view of a contiguous (N, H, W, 3) uint8 frame"
+        assert lut is not None and lut.dtype == torch.float16 and lut.numel() == 768 and lut.is_contiguous()
+        kind = 2
+    else:
+        assert x.dtype in (torch.float32, torch.float16) and x.is_contiguous()
+        kind = 0 if x.dtype == torch.float32 else 1
+    assert w0.dtype == torch.float32 and w0.is_contiguous() and tuple(w0.shape[1:]) == (3, 3, 3)
+    C0 = w0.shape[0]
+    H1, W1 = conv_out_size((H + 1) // 2, (W + 1) // 2, 3, 2, 1)
+    if out is None:
+        out = empty_nhwc(N, C1, H1, W1, x.device)
+    _, _, _, _, ycs = nhwc_info(out)
+    assert tuple(out.shape) == (N, C1, H1, W1), (tuple(out.shape), (N, C1, H1, W1))
+    rc = _lib.lib().fsb_stem_fused(N, H, W, kind, _ptr(x), _ptr(lut if kind == 2 else None), C0, _ptr(w0), _ptr(scale0), _ptr(shift0),
+                                   C1, _ptr(w1_packed), _ptr(scale1), _ptr(shift1), _ptr(out), ycs, _stream())
+    if rc == _lib.FSB_ERR_UNSUPPORTED:
+        return None
+    check(rc, "fsb_stem_fused")
+    return out
+
+
 def confusion_matrix(pred_u8, gt, n_cl, out=None):
     """accumulate hist_info (tools/seg_opr/metric.py:7-15) of `pred_u8` vs `gt` into the int64 [n_cl^2 + 2] tensor `out`"""
     assert pred_u8.dtype == torch.uint8 and pred_u8.is_contiguous() and gt.is_contiguous() and pred_u8.numel() == gt.numel()

@@ -25,6 +25,7 @@ Without a GPU (tests) the same code runs the passes eagerly (capture=False) on t
 from __future__ import annotations
 
 import ctypes as C
+import gc
 import os
 import weakref
 
@@ -381,6 +382,12 @@ class PassContext:
         self.g_pack, self.g_fwd, self.g_bwd = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
         torch.cuda.synchronize()
         self._capturing = True
+        # No automatic garbage collection while capturing: an unreachable earlier pass whose graphs the cyclic collector frees in
+        # the middle of a capture destroys them while a stream is capturing, which invalidates this capture.  Collect first, so
+        # that such passes are freed here instead.
+        gc.collect()
+        gc_enabled = gc.isenabled()
+        gc.disable()
         try:
             with torch.cuda.graph(self.g_pack, pool=pool):
                 self._repack()
@@ -390,6 +397,8 @@ class PassContext:
                 self.dW, self.dB = self._run_backward(self._tape, self.outs, self.dlogits)
         finally:
             self._capturing = False
+            if gc_enabled:
+                gc.enable()
         self.graphs = (self.g_pack, self.g_fwd, self.g_bwd)
 
     # ---- per-step execution ----------------------------------------------------------------------------------------

@@ -20,6 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import decode
+from . import engine
 from . import functional as F_
 from .decode import (alphas2ops_path_width, betas2path, downs2path, network_metas, path2downs, path2widths,  # noqa: F401
                      softmax)
@@ -239,11 +240,43 @@ class Network_Multi_Path_Infer(nn.Module):
             self.__dict__["_fsb_streams"] = streams
         return streams
 
+    def _stem(self, input):
+        """self.stem(input).  At inference on a CUDA input, stem.0 and the first conv of stem.1 run as one kernel
+        (F_.stem_fused), so the 1/2-resolution map never goes through HBM; the rest of the stem runs unchanged.  Anything the
+        fused kernel was not written for -- training, autograd, other stem layers or widths -- runs self.stem as before."""
+        stem0, stem1 = self.stem[0], self.stem[1]
+        if (self.training or torch.is_grad_enabled() or not input.is_cuda or type(stem0) is not ConvNorm
+                or type(stem1) is not BasicResidual2x):
+            return self.stem(input)
+        conv0, bn0, conv1, bn1 = stem0.conv[0], stem0.conv[1], stem1.conv1, stem1.bn1
+        lut = None
+        if input.dtype == torch.uint8:
+            lut = stem0.__dict__.get("_fsb_norm_lut")
+            usable = lut is not None
+        else:
+            usable = input.dtype in (torch.float32, torch.float16) and input.is_contiguous() and not F_.is_nhwc_half(input)
+        usable = usable and (stem0.C_in == 3 and stem0.kernel_size == 3 and stem0.stride == 2 and stem0.padding == 1
+                             and not stem0.slimmable and conv0.bias is None and not bn0.training)
+        usable = usable and (not stem1.slimmable and conv1.kernel_size[0] == 3 and conv1.stride[0] == 2 and conv1.padding[0] == 1
+                             and conv1.dilation[0] == 1 and conv1.groups == 1 and not bn1.training and not stem1.bn2.training)
+        if not usable:
+            return self.stem(input)
+        scale0, shift0 = engine.folded_bn(bn0, stem0.C_out, None)
+        w0 = conv0.weight.detach()
+        ci, co = engine.active_channels(conv1)
+        scale1, shift1 = engine.folded_bn(engine.active_bn(bn1), co, conv1.bias)
+        y = F_.stem_fused(input, lut, w0 if w0.dtype == torch.float32 else w0.float(), scale0, shift0,
+                          engine.packed_weight(conv1, ci, co), co, scale1, shift1)
+        if y is None:
+            return self.stem(input)
+        y = engine.conv_bn_act(y, stem1.conv2, stem1.bn2, relu=True)
+        return self.stem[2](y)
+
     def _trunk(self, input, ctx=None):
         """stem + cells -> per scale, the latest feature of every branch ({8: [...], 16: [...], 32: [...]})"""
         full_h = input.size(2)
         ctx = ctx if ctx is not None else _BranchCtx(None)
-        stem = self.stem(input)
+        stem = self._stem(input)
         # The concat buffer that the side streams will write into is allocated on the main stream BEFORE the fork, so the
         # block the caching allocator hands out cannot still be in use by main-stream work the side streams do not wait for.
         f8 = self.num_filters(8, self._stem_head_width[1])

@@ -39,6 +39,18 @@ def _rec_stem(res, a, kw):
             "bytes": float(x.numel() * _esize(x) + N * Co * Ho * Wo * 2 + w.numel() * 4), "shape": "3x3 3->%d @%dx%d s2" % (Co, Ho, Wo)}
 
 
+def _rec_stem_fused(res, a, kw):
+    x, w0, w1 = a[0], a[2], a[5]
+    if res is None:   # no fused kernel for these widths: the caller's two launches are recorded instead
+        return None
+    N, C1, H1, W1 = res.shape
+    C0 = w0.shape[0]
+    H0, W0 = (x.shape[2] + 1) // 2, (x.shape[3] + 1) // 2
+    return {"kernel": "stem_fused", "flops": 2.0 * 27 * C0 * N * H0 * W0 + 2.0 * 9 * C0 * C1 * N * H1 * W1,
+            "bytes": float(x.numel() * _esize(x) + N * C1 * H1 * W1 * 2 + w0.numel() * 4 + w1.numel() * 2),
+            "shape": "3x3 3->%d->%d @%dx%d s2 s2" % (C0, C1, H1, W1)}
+
+
 def _rec_bilinear(res, a, kw):
     x = a[0]
     N, Cc, Hi, Wi = x.shape
@@ -65,7 +77,7 @@ def _rec_argmax(res, a, kw):
             "shape": "%d ch %dx%d -> %dx%d u8" % (x.shape[1], x.shape[2], x.shape[3], res.shape[1], res.shape[2])}
 
 
-_RECORDERS = {"conv_fwd": _rec_conv, "stem_conv_nchw": _rec_stem, "bilinear": _rec_bilinear, "copy_channels": _rec_copy,
+_RECORDERS = {"conv_fwd": _rec_conv, "stem_conv_nchw": _rec_stem, "stem_fused": _rec_stem_fused, "bilinear": _rec_bilinear, "copy_channels": _rec_copy,
               "upsample_logits": _rec_upsample, "upsample_argmax": _rec_argmax}
 
 
@@ -76,7 +88,9 @@ def _instrumented(records: List[Dict]):
     def traced(orig, make_record):
         def call(*a, **kw):
             res = orig(*a, **kw)
-            records.append(make_record(res, a, kw))
+            rec = make_record(res, a, kw)
+            if rec is not None:
+                records.append(rec)
             return res
         return call
 

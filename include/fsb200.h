@@ -164,6 +164,17 @@ int fsb_stem_conv_nchw(int N, int H, int W, int Cout, const void* x_nchw, int x_
  * Bit-identical to fsb_stem_conv_nchw on the normalised fp32 frame; the host->device copy is 4x smaller. */
 int fsb_stem_conv_u8hwc(int N, int H, int W, int Cout, const uint8_t* x_hwc, const void* lut_f16, const float* w,
                         const float* scale, const float* shift, void* y, int y_cstride, uint32_t flags, void* stream);
+/* The stem's first two convs as one kernel: stem.0 (the RGB ConvNorm above, C0 output channels) followed by conv1 of the stride-2
+ * BasicResidual2x stem.1 (3x3 stride 2 pad 1, C0 -> C1) with its BN(eval) + ReLU, without writing the 1/2-resolution map
+ * (ConvNorm at train/model_seg.py:193, BasicResidual2x at search/operations.py:280-359).  in_kind: 0 = fp32 NCHW, 1 = fp16 NCHW,
+ * 2 = uint8 HWC with lut_f16 as in fsb_stem_conv_u8hwc.  w0: fp32 OIHW [C0][3][3][3]; w1_packed: fsb_pack_conv_weight's layout of
+ * the C0 -> C1 weight; scale / shift: folded BN of each conv.  y: fp16 NHWC 1/4-resolution map with channel stride y_cstride.
+ * Bit-identical to fsb_stem_conv_nchw / fsb_stem_conv_u8hwc (AFFINE | RELU) followed by fsb_conv_fwd (AFFINE | RELU).
+ * FSB_ERR_UNSUPPORTED unless 16 <= C0 <= 32, C1 == 64, y_cstride % 8 == 0 and w1_packed, y 16-byte aligned (the student's stem);
+ * the caller then runs the two kernels. */
+int fsb_stem_fused(int N, int H, int W, int in_kind, const void* x, const void* lut_f16, int C0, const float* w0, const float* scale0,
+                   const float* shift0, int C1, const void* w1_packed, const float* scale1, const float* shift1, void* y, int y_cstride,
+                   void* stream);
 /* Evaluator's confusion matrix on the device (tools/seg_opr/metric.py:7-15 hist_info): for the n pixels with 0 <= gt < n_cl:
  * out[n_cl * gt + pred] += 1, out[n_cl^2] += 1 (labeled), out[n_cl^2 + 1] += (pred == gt) (correct).  out: int64
  * [n_cl * n_cl + 2], accumulated into (caller zeroes once per evaluation); gt: uint8 / int32 / int64 (gt_bytes = 1 / 4 / 8). */
