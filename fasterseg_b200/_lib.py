@@ -63,6 +63,7 @@ _SIGS = {
     "fsb_bilinear_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, C.c_uint32, _P]),
     "fsb_upsample_logits_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_argmax": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),
+    "fsb_upsample_argmax_confusion": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P, _P]),
     "fsb_nearest_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_logits_nearest_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_argmax_nearest": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),

@@ -103,6 +103,7 @@ int confusion_launch(int64_t, const uint8_t*, const void*, int, int, long long*,
 int bilinear_launch(int, int, int, int, int, int, const void*, int, void*, int, uint32_t, cudaStream_t);
 int upsample_logits_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
+int upsample_argmax_confusion_launch(int, int, int, int, int, int, const void*, int, const void*, int, long long*, cudaStream_t);
 int nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_logits_nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_nearest_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
@@ -346,6 +347,12 @@ int fsb_upsample_logits_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const
 int fsb_upsample_argmax(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, uint8_t* labels, void* stream) {
   if (N <= 0 || C <= 0 || C > 255 || !x || !labels || xcs < C) return set_error(FSB_ERR_INVALID, "upsample_argmax: bad argument");
   return upsample_argmax_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, labels, static_cast<cudaStream_t>(stream));
+}
+int fsb_upsample_argmax_confusion(int N, int n_cl, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, const void* gt, int gt_bytes,
+                                  long long* out, void* stream) {
+  if (N <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !gt || !out || xcs < n_cl)
+    return set_error(FSB_ERR_INVALID, "upsample_argmax_confusion: bad argument");
+  return upsample_argmax_confusion_launch(N, n_cl, Hi, Wi, Ho, Wo, x, xcs, gt, gt_bytes, out, static_cast<cudaStream_t>(stream));
 }
 
 int fsb_nearest_fwd(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int ycs, void* stream) {

@@ -424,20 +424,12 @@ int upsample_logits_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const v
 }
 
 // ------------------------------------------------------------------------------------------
-// fused upsample + argmax -> uint8 labels.  One thread = 4 consecutive output columns (one 32-bit store).
+// fused upsample + argmax.  One work item = 4 consecutive output columns wv*4.. of output row ho of image n: the argmax over
+// the C classes of the bilinear (align_corners) value at each.  Columns past Wo repeat the last column.  Both the label kernel
+// and the confusion kernel below call this, so their labels are the same bits.
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128)
-upsample_argmax_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs,
-                       uint8_t* __restrict__ labels, float sh, float sw) {
-  pdl_launch_dependents();
-  pdl_wait();
-  const int wvec = (Wo + 3) >> 2;
-  const int64_t total = static_cast<int64_t>(N) * Ho * wvec;
-  const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
-  if (gid >= total) return;
-  const int wv = static_cast<int>(gid % wvec);
-  const int ho = static_cast<int>((gid / wvec) % Ho);
-  const int n = static_cast<int>(gid / (static_cast<int64_t>(wvec) * Ho));
+__device__ __forceinline__ void upsample_argmax4(int C, int Hi, int Wi, int Wo, const __half* __restrict__ x, int xcs, float sh,
+                                                 float sw, int n, int ho, int wv, int (&arg)[4]) {
   int h0, h1;
   float lh;
   src_index(ho, sh, Hi, h0, h1, lh);
@@ -448,7 +440,8 @@ upsample_argmax_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __hal
 #pragma unroll
   for (int j = 0; j < 4; ++j) src_index(min(wv * 4 + j, Wo - 1), sw, Wi, w0[j], w1[j], lw[j]);
   float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-  int arg[4] = {0, 0, 0, 0};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) arg[j] = 0;
   for (int c = 0; c < C; ++c) {
     int prev = -1;
     float a0 = 0.f, a1 = 0.f;
@@ -470,6 +463,23 @@ upsample_argmax_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __hal
       }
     }
   }
+}
+
+// -> uint8 labels.  One thread = 4 consecutive output columns (one 32-bit store).
+__global__ void __launch_bounds__(128)
+upsample_argmax_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs,
+                       uint8_t* __restrict__ labels, float sh, float sw) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int wvec = (Wo + 3) >> 2;
+  const int64_t total = static_cast<int64_t>(N) * Ho * wvec;
+  const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (gid >= total) return;
+  const int wv = static_cast<int>(gid % wvec);
+  const int ho = static_cast<int>((gid / wvec) % Ho);
+  const int n = static_cast<int>(gid / (static_cast<int64_t>(wvec) * Ho));
+  int arg[4];
+  upsample_argmax4(C, Hi, Wi, Wo, x, xcs, sh, sw, n, ho, wv, arg);
   uint8_t* dst = labels + (static_cast<size_t>(n) * Ho + ho) * Wo + wv * 4;
   if (wv * 4 + 4 <= Wo && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
     *reinterpret_cast<uint32_t*>(dst) = static_cast<uint32_t>(arg[0]) | (static_cast<uint32_t>(arg[1]) << 8) |
@@ -489,6 +499,78 @@ int upsample_argmax_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const v
                                                                          xcs, labels, ac_scale(Hi, Ho), ac_scale(Wi, Wo));
   cudaError_t e = last_launch_error();
   if (e != cudaSuccess) return set_cuda_error(e, "upsample_argmax launch");
+  return FSB_OK;
+}
+
+// upsample + argmax + confusion matrix (tools/seg_opr/metric.py:7-15 hist_info) without writing the label map: the labels of
+// upsample_argmax4 go straight into a per-CTA shared-memory histogram, flushed with integer atomics (exact, order-independent).
+// Counting rule of confusion_kernel (conv_direct.cu): gt outside [0, n_cl) is ignored, hist[n_cl * gt + pred] += 1,
+// labeled += 1, correct += (pred == gt).  out: int64 [n_cl * n_cl + 2], accumulated into.  Grid-stride over the work items.
+template <typename TGt>
+__global__ void __launch_bounds__(256)
+upsample_argmax_confusion_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs,
+                                 const TGt* __restrict__ gt, float sh, float sw, unsigned long long* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ unsigned int s_cm[];  // C * C + 2
+  const int cells = C * C + 2;
+  for (int i = threadIdx.x; i < cells; i += blockDim.x) s_cm[i] = 0;
+  __syncthreads();
+  const int wvec = (Wo + 3) >> 2;
+  const int64_t total = static_cast<int64_t>(N) * Ho * wvec;
+  unsigned int labeled = 0, correct = 0;
+  for (int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; gid < total;
+       gid += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int wv = static_cast<int>(gid % wvec);
+    const int ho = static_cast<int>((gid / wvec) % Ho);
+    const int n = static_cast<int>(gid / (static_cast<int64_t>(wvec) * Ho));
+    int arg[4];
+    upsample_argmax4(C, Hi, Wi, Wo, x, xcs, sh, sw, n, ho, wv, arg);
+    const TGt* g = gt + (static_cast<size_t>(n) * Ho + ho) * Wo + wv * 4;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      if (wv * 4 + j >= Wo) break;
+      const long long t = static_cast<long long>(g[j]);
+      if (t < 0 || t >= C) continue;
+      atomicAdd(&s_cm[t * C + arg[j]], 1u);
+      ++labeled;
+      correct += arg[j] == t ? 1u : 0u;
+    }
+  }
+  if (labeled) atomicAdd(&s_cm[C * C], labeled);
+  if (correct) atomicAdd(&s_cm[C * C + 1], correct);
+  __syncthreads();
+  for (int i = threadIdx.x; i < cells; i += blockDim.x)
+    if (s_cm[i]) atomicAdd(&out[i], static_cast<unsigned long long>(s_cm[i]));
+}
+
+int upsample_argmax_confusion_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, const void* gt, int gt_bytes,
+                                     long long* out, cudaStream_t stream) {
+  if (C < 1 || C > 64) return set_error(FSB_ERR_INVALID, "upsample_argmax_confusion: 1 <= n_cl <= 64");
+  const int64_t total = static_cast<int64_t>(N) * Ho * ((Wo + 3) / 4);
+  // at most 4 CTAs per SM (2 are resident at this kernel's register count): large maps run several work items per thread, which
+  // amortises the histogram's clear and flush
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > static_cast<int64_t>(sm_count()) * 4) blocks = static_cast<int64_t>(sm_count()) * 4;
+  if (blocks < 1) blocks = 1;
+  const size_t smem = static_cast<size_t>(C * C + 2) * sizeof(unsigned int);
+  const __half* xh = static_cast<const __half*>(x);
+  const float sh = ac_scale(Hi, Ho), sw = ac_scale(Wi, Wo);
+  unsigned long long* o = reinterpret_cast<unsigned long long*>(out);
+  const dim3 grid(static_cast<unsigned>(blocks));
+  if (gt_bytes == 1)
+    FSB_LAUNCH(upsample_argmax_confusion_kernel<uint8_t>, grid, dim3(256), smem, stream, N, C, Hi, Wi, Ho, Wo, xh, xcs,
+               static_cast<const uint8_t*>(gt), sh, sw, o);
+  else if (gt_bytes == 4)
+    FSB_LAUNCH(upsample_argmax_confusion_kernel<int32_t>, grid, dim3(256), smem, stream, N, C, Hi, Wi, Ho, Wo, xh, xcs,
+               static_cast<const int32_t*>(gt), sh, sw, o);
+  else if (gt_bytes == 8)
+    FSB_LAUNCH(upsample_argmax_confusion_kernel<long long>, grid, dim3(256), smem, stream, N, C, Hi, Wi, Ho, Wo, xh, xcs,
+               static_cast<const long long*>(gt), sh, sw, o);
+  else
+    return set_error(FSB_ERR_INVALID, "upsample_argmax_confusion: ground truth must be uint8, int32 or int64");
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "upsample_argmax_confusion launch");
   return FSB_OK;
 }
 

@@ -369,6 +369,25 @@ def upsample_argmax(x, size, out=None):
     return out
 
 
+def upsample_argmax_confusion(x, size, gt, n_cl, out):
+    """confusion_matrix(upsample_argmax(x, size), gt, n_cl, out) in one launch that never writes the label map: x holds the n_cl
+    class logits (NHWC fp16 view), gt the N x Ho x Wo ground truth (uint8 / int32 / int64, values outside [0, n_cl) ignored), out the
+    int64 [n_cl^2 + 2] counters, accumulated into.  The counters are bit-identical to the two-kernel path."""
+    N, Cc, Hi, Wi, xcs = nhwc_info(x)
+    Ho, Wo = int(size[0]), int(size[1])
+    n_cl = int(n_cl)
+    if Cc != n_cl:
+        raise ValueError("upsample_argmax_confusion: logits have %d classes, n_cl is %d" % (Cc, n_cl))
+    if gt.dtype not in (torch.uint8, torch.int32, torch.int64) or not gt.is_contiguous() or gt.numel() != N * Ho * Wo or not _on_device(gt):
+        raise ValueError("upsample_argmax_confusion: gt must be a contiguous CUDA uint8 / int32 / int64 tensor of %d x %d x %d elements, "
+                         "got %s %s" % (N, Ho, Wo, gt.dtype, tuple(gt.shape)))
+    if out.dtype != torch.int64 or not out.is_contiguous() or out.numel() != n_cl * n_cl + 2 or not _on_device(out):
+        raise ValueError("upsample_argmax_confusion: out must be a contiguous CUDA int64 tensor of n_cl^2 + 2 elements")
+    check(_lib.lib().fsb_upsample_argmax_confusion(N, n_cl, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(gt), gt.element_size(), _ptr(out),
+                                                   _stream()), "fsb_upsample_argmax_confusion")
+    return out
+
+
 def nearest(x, size, out=None):
     """F.interpolate(x, size, mode='nearest') on NHWC fp16 views (torch's legacy index rule; a copy, so bit-exact)"""
     N, Cc, Hi, Wi, xcs = nhwc_info(x)

@@ -77,3 +77,9 @@ class Network_Multi_Path_Infer(_train.Network_Multi_Path_Infer):
         self._inference_only(input)
         pred8 = self._features(input)
         return F_.upsample_argmax_nearest(pred8, (int(pred8.size(2)) * 8, int(pred8.size(3)) * 8), out=out)
+
+    @torch.no_grad()
+    def accumulate_confusion(self, input, gt, cm):
+        """hist_info of predict_labels(input) against `gt` into `cm` (metric.ConfusionMatrix); the fused kernel of the train/
+        network is bilinear, so the nearest labels go through the label map"""
+        cm.update(self.predict_labels(input), gt)

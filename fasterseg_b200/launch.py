@@ -217,6 +217,54 @@ def install_data_parallel():
     return _Lazy([]).install()
 
 
+def reference_tools_dir(script):
+    """<FasterSeg>/tools for a driver at <FasterSeg>/<dir>/<script>.py (config_*.py puts the same directory on sys.path), or None"""
+    tools = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(script))), "tools")
+    return tools if os.path.isfile(os.path.join(tools, "engine", "evaluator.py")) else None
+
+
+class _PatchAfterImport:
+    """sys.meta_path finder: when `name` is imported from `origin`, loads it with its own loader and then calls patch(module)"""
+
+    def __init__(self, name, origin, patch):
+        self.name, self.origin, self.patch = name, os.path.realpath(origin), patch
+
+    def find_spec(self, fullname, path=None, target=None):
+        if fullname != self.name:
+            return None
+        from importlib.machinery import PathFinder
+        spec = PathFinder.find_spec(fullname, path)
+        if spec is None or spec.origin is None or os.path.realpath(spec.origin) != self.origin:
+            return None
+        spec.loader = _PatchingLoader(spec.loader, self.patch)
+        return spec
+
+
+class _PatchingLoader:
+    def __init__(self, loader, patch):
+        self.loader, self.patch = loader, patch
+
+    def create_module(self, spec):
+        return self.loader.create_module(spec)
+
+    def exec_module(self, module):
+        self.loader.exec_module(module)
+        self.patch(module)
+
+
+def install_evaluator_patch(script):
+    """Validation on the device (fasterseg_b200.evaluator): when the driver imports the reference's engine.evaluator from the
+    tools/ directory next to its own, patch Evaluator.run_online / run_online_multiprocess.  Returns the finder, or None (and
+    changes nothing) when no reference tools/ directory is found."""
+    tools = reference_tools_dir(script)
+    if tools is None:
+        return None
+    from . import evaluator
+    finder = _PatchAfterImport("engine.evaluator", os.path.join(tools, "engine", "evaluator.py"), evaluator.install)
+    sys.meta_path.insert(0, finder)
+    return finder
+
+
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     if not argv:
@@ -227,6 +275,7 @@ def main(argv=None):
     install_compat_patches()
     install_shadow_modules(script)
     install_data_parallel()
+    install_evaluator_patch(script)
     from . import optim
     optim.install()      # torch.optim.SGD / nn.utils.clip_grad_norm_ take the flat path after a captured `_loss` (torch's otherwise)
     sys.argv = argv

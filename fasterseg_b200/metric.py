@@ -19,6 +19,11 @@ class ConfusionMatrix:
         """pred_u8: uint8 label map(s); gt: same number of elements, uint8 / int32 / int64 (255 or negative = ignore)"""
         F_.confusion_matrix(pred_u8.contiguous(), gt.contiguous(), self.n_cl, out=self.acc)
 
+    def update_from_logits(self, logits, size, gt):
+        """accumulate hist_info of argmax(upsample(logits, size)) vs gt in one kernel, without a label map: `logits` are the
+        low-resolution NHWC fp16 class scores (n_cl channels), bilinear align_corners=True to `size` = gt's (H, W)"""
+        F_.upsample_argmax_confusion(logits, size, gt.contiguous(), self.n_cl, self.acc)
+
     def result(self):
         """-> (hist [n_cl, n_cl] int64, labeled, correct) like metric.hist_info summed over the images seen"""
         a = self.acc.cpu().numpy()

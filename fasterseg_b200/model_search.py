@@ -300,9 +300,10 @@ class Network_Multi_Path(nn.Module):
             return AG.run_taped(self, self._forward, input)   # EXPERIMENTAL: the whole pass as one autograd node
         return self._forward(input)
 
-    def _forward(self, input, plan=None):
+    def _forward(self, input, plan=None, head=None):
         """plan (graphed.PassContext): a captured pass -- mixing weights and widths come from static device slots instead of being
-        computed here; the tensor work is identical."""
+        computed here; the tensor work is identical.  head (eval, no plan): return only that head's 1/8 NHWC logits, running only
+        the refine chains it reads; widths are drawn exactly as for the full pass."""
         idx = self.arch_idx
         refine16, refine32 = self.refine16[idx], self.refine32[idx]
         if plan is None:
@@ -347,11 +348,41 @@ class Network_Multi_Path(nn.Module):
             return refine32[3](_cat([_resize2x(refine32[2](o)), f8]))
 
         out0 = f8
+        heads = [lambda: self.head0[idx](out0), lambda: self.head1[idx](out1), lambda: self.head2[idx](out2),
+                 lambda: self.head02[idx](_cat([out0, out2])), lambda: self.head12[idx](_cat([out1, out2]))]
+        if head is not None:
+            out1 = chain16() if head in (1, 4) else None
+            out2 = chain32() if head in (2, 3, 4) else None
+            return heads[head]()
         out1, out2 = fan([chain16, chain32])
-        preds = fan([lambda: self.head0[idx](out0), lambda: self.head1[idx](out1), lambda: self.head2[idx](out2),
-                     lambda: self.head02[idx](_cat([out0, out2])), lambda: self.head12[idx](_cat([out1, out2]))])
+        preds = fan(heads)
         leave = _to_nchw if self.training else _upsample8
         return tuple(leave(p) for p in preds)
+
+    def set_input_normalization(self, mean, std):
+        """After this every architecture's stem also accepts the uint8 HWC image itself, passed as `img_u8.permute(0, 3, 1, 2)`,
+        and applies (v / 255 - mean) / std in its gather (Network_Multi_Path_Infer.set_input_normalization)"""
+        lut = F_.normalization_lut(mean, std, next(self.parameters()).device)
+        for stem in self.stem:
+            stem[0].__dict__["_fsb_norm_lut"] = lut
+
+    def _head_logits(self, input, head):
+        assert not self.training and 0 <= int(head) < 5
+        return F_.to_nhwc_half(self._forward(input, head=int(head)))
+
+    @torch.no_grad()
+    def predict_labels(self, input, head=0):
+        """argmax(forward(input)[head], dim=1) as uint8 (the evaluator's `score[out_idx]` -> exp -> argmax,
+        tools/engine/evaluator.py:306-318): the eval forward with that head only, and the fused x8 upsample + argmax"""
+        p = self._head_logits(input, head)
+        return F_.upsample_argmax(p, (int(p.size(2)) * 8, int(p.size(3)) * 8))
+
+    @torch.no_grad()
+    def accumulate_confusion(self, input, gt, cm, head=0):
+        """hist_info of predict_labels(input, head) against `gt` into `cm` (metric.ConfusionMatrix), in one kernel after the
+        eval forward and without a label map"""
+        p = self._head_logits(input, head)
+        cm.update_from_logits(p, (int(p.size(2)) * 8, int(p.size(3)) * 8), gt)
 
     def forward_latency(self, size, alpha=True, beta=True, ratio=True):
         """Expected latency of the current architecture distribution from the per-op lookup table

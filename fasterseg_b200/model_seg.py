@@ -391,6 +391,15 @@ class Network_Multi_Path_Infer(nn.Module):
         pred8 = self._features(input)
         return F_.upsample_argmax(pred8, (int(pred8.size(2)) * 8, int(pred8.size(3)) * 8), out=out)
 
+    @torch.no_grad()
+    def accumulate_confusion(self, input, gt, cm):
+        """Validation of one batch (tools/engine/evaluator.py:297-318 + tools/seg_opr/metric.py:7-15): the eval forward to the 1/8
+        logits, then one kernel upsamples, takes the argmax and adds hist_info against `gt` (N x H x W) into `cm`
+        (metric.ConfusionMatrix).  The counters equal those of predict_labels followed by cm.update."""
+        assert not self.training
+        pred8 = self._features(input)
+        cm.update_from_logits(pred8, (int(pred8.size(2)) * 8, int(pred8.size(3)) * 8), gt)
+
     # ---------------------------------------------------------------------------------------------------------
     # latency model (table lookups, model_seg.py:368-408)
     # ---------------------------------------------------------------------------------------------------------

@@ -194,6 +194,12 @@ int fsb_upsample_logits_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const
  * torch.argmax / np.argmax at tools/engine/evaluator.py:315-318). */
 int fsb_upsample_argmax(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, uint8_t* labels,
                         void* stream);
+/* The two above fused for validation (tools/engine/evaluator.py:297-318 + tools/seg_opr/metric.py:7-15): fsb_upsample_argmax of
+ * the n_cl-class logits x, then fsb_confusion_matrix of those labels against gt [N, Ho, Wo] (uint8 / int32 / int64, gt_bytes =
+ * 1 / 4 / 8; values outside [0, n_cl) are ignored), accumulated into out (int64 [n_cl * n_cl + 2], same layout).  The label
+ * map is never written.  Bit-identical counters to the two calls; 1 <= n_cl <= 64. */
+int fsb_upsample_argmax_confusion(int N, int n_cl, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, const void* gt,
+                                  int gt_bytes, long long* out, void* stream);
 /* F.interpolate(mode='nearest') (torch's legacy rule, not 'nearest-exact') on fp16 NHWC channel slices (latency/ network,
  * latency/operations.py:265,269,427,434, latency/model_seg.py:305,309,315).  Per axis
  *   src = min((int)floorf((float)dst * ((float)in / (float)out)), in - 1)   in fp32, exactly as torch computes it.
