@@ -37,6 +37,11 @@ class BnSel(C.Structure):
                 ("reserved", C.c_int32)]
 
 
+class TrainPreDesc(C.Structure):
+    """fsb_train_pre_desc: batch geometry of the training augmentation"""
+    _fields_ = [(n, C.c_int32) for n in ("n", "crop_h", "crop_w", "label_h", "label_w")]
+
+
 _P = C.c_void_p
 _SIGS = {
     "fsb_abi_version": (C.c_int, []),
@@ -125,6 +130,7 @@ _SIGS = {
     "fsb_supernet_latency_workspace_bytes": (C.c_size_t, [_P]),
     "fsb_supernet_latency_fwd": (C.c_int, [_P] * 13 + [_P]),
     "fsb_supernet_latency_bwd": (C.c_int, [_P] * 12 + [_P]),
+    "fsb_train_pre": (C.c_int, [C.POINTER(TrainPreDesc)] + [_P] * 7),
 }
 EXPORTED_SYMBOLS = tuple(_SIGS)
 

@@ -6,7 +6,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libfsb200.so")
-SOURCES = ["api.cu", "conv_tc.cu", "conv_direct.cu", "resize.cu", "bn.cu", "train.cu", "wgrad_tc.cu", "train_fused.cu", "loss.cu", "optim.cu", "dp.cu", "peer.cu", "latency.cu", "stem_fused.cu"]
+SOURCES = ["api.cu", "conv_tc.cu", "conv_direct.cu", "resize.cu", "bn.cu", "train.cu", "wgrad_tc.cu", "train_fused.cu", "loss.cu", "optim.cu", "dp.cu", "peer.cu", "latency.cu", "stem_fused.cu", "trainpre.cu"]
 HEADERS = ["fsb_common.cuh", "fsb_internal.h", os.path.join("..", "..", "include", "fsb200.h")]
 
 

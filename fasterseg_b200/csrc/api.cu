@@ -104,6 +104,8 @@ int bilinear_launch(int, int, int, int, int, int, const void*, int, void*, int, 
 int upsample_logits_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
 int upsample_argmax_confusion_launch(int, int, int, int, int, int, const void*, int, const void*, int, long long*, cudaStream_t);
+int train_pre_launch(const fsb_train_pre_desc&, const uint8_t*, const uint8_t*, const int32_t*, const float*, float*, long long*,
+                     cudaStream_t);
 int nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_logits_nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_nearest_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
@@ -353,6 +355,13 @@ int fsb_upsample_argmax_confusion(int N, int n_cl, int Hi, int Wi, int Ho, int W
   if (N <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !gt || !out || xcs < n_cl)
     return set_error(FSB_ERR_INVALID, "upsample_argmax_confusion: bad argument");
   return upsample_argmax_confusion_launch(N, n_cl, Hi, Wi, Ho, Wo, x, xcs, gt, gt_bytes, out, static_cast<cudaStream_t>(stream));
+}
+int fsb_train_pre(const fsb_train_pre_desc* d, const uint8_t* img, const uint8_t* gt, const int32_t* geom, const float* lut,
+                  float* out_img, int64_t* out_gt, void* stream) {
+  if (!d || d->n <= 0 || d->n > 65535 || d->crop_h <= 0 || d->crop_h > 65535 || d->crop_w <= 0 || d->label_h <= 0 ||
+      d->label_h > d->crop_h || d->label_w <= 0 || d->label_w > d->crop_w || !img || !gt || !geom || !lut || !out_img || !out_gt)
+    return set_error(FSB_ERR_INVALID, "train_pre: bad argument");
+  return train_pre_launch(*d, img, gt, geom, lut, out_img, reinterpret_cast<long long*>(out_gt), static_cast<cudaStream_t>(stream));
 }
 
 int fsb_nearest_fwd(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int ycs, void* stream) {

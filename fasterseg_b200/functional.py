@@ -278,6 +278,43 @@ def confusion_matrix(pred_u8, gt, n_cl, out=None):
     return out
 
 
+TRAIN_PRE_GEOM = 8   # int32 per image: H, W, mirror, sh, sw, pos_h, pos_w, pixel offset (fasterseg_b200/trainpre.py builds them)
+
+
+def train_pre(img, gt, geom, lut, crop, label_size, out_img=None, out_gt=None):
+    """TrainPre (train/dataloader.py:14-31) of a batch on the device, bit-identical to the reference: img / gt are the packed uint8
+    HWC RGB sources and uint8 labels, geom the int32 [N, 8] geometry records (validated on the host by trainpre.check_geometry),
+    lut the float32 [3, 256] normalisation table, crop = (image_height, image_width), label_size = the label map's (h, w).
+    -> (float32 [N, 3, crop_h, crop_w], int64 [N, label_h, label_w])"""
+    if geom.dtype != torch.int32 or geom.dim() != 2 or geom.shape[1] != TRAIN_PRE_GEOM or not geom.is_contiguous():
+        raise ValueError("train_pre: geom must be a contiguous int32 [N, %d] tensor, got %s %s"
+                         % (TRAIN_PRE_GEOM, geom.dtype, tuple(geom.shape)))
+    for name, t in (("img", img), ("gt", gt)):
+        if t.dtype != torch.uint8 or not t.is_contiguous():
+            raise ValueError("train_pre: %s must be a contiguous uint8 tensor" % name)
+    if lut.dtype != torch.float32 or lut.numel() != 3 * 256 or not lut.is_contiguous():
+        raise ValueError("train_pre: lut must be a contiguous float32 [3, 256] tensor")
+    N = geom.shape[0]
+    ch, cw = int(crop[0]), int(crop[1])
+    lh, lw = int(label_size[0]), int(label_size[1])
+    if out_img is None:
+        out_img = torch.empty(N, 3, ch, cw, dtype=torch.float32, device=img.device)
+    if out_gt is None:
+        out_gt = torch.empty(N, lh, lw, dtype=torch.int64, device=img.device)
+    if out_img.dtype != torch.float32 or tuple(out_img.shape) != (N, 3, ch, cw) or not out_img.is_contiguous():
+        raise ValueError("train_pre: out_img must be a contiguous float32 [%d, 3, %d, %d] tensor" % (N, ch, cw))
+    if out_gt.dtype != torch.int64 or tuple(out_gt.shape) != (N, lh, lw) or not out_gt.is_contiguous():
+        raise ValueError("train_pre: out_gt must be a contiguous int64 [%d, %d, %d] tensor" % (N, lh, lw))
+    if not all(_on_device(t) for t in (img, gt, geom, lut, out_img, out_gt)):
+        raise ValueError("train_pre: every tensor must be on the GPU")
+    if len({t.device for t in (img, gt, geom, lut, out_img, out_gt)}) != 1:
+        raise ValueError("train_pre: every tensor must be on the same device")
+    desc = _lib.TrainPreDesc(N, ch, cw, lh, lw)
+    check(_lib.lib().fsb_train_pre(C.byref(desc), _ptr(img), _ptr(gt), _ptr(geom), _ptr(lut), _ptr(out_img), _ptr(out_gt), _stream()),
+          "fsb_train_pre")
+    return out_img, out_gt
+
+
 # ---- flat step tail (csrc/optim.cu): tables are built by optim.FlatTables ---------------------------------------------------------
 def flat_chunk() -> int:
     """elements of one block of the flat kernels' block map"""

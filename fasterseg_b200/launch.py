@@ -265,6 +265,19 @@ def install_evaluator_patch(script):
     return finder
 
 
+def install_dataloader_patch(script):
+    """Training augmentation on the device (fasterseg_b200.trainpre): when the driver imports the `dataloader` module next to it
+    (train/dataloader.py, search/dataloader.py), wrap its get_train_loader.  Returns the finder, or None (and changes nothing)
+    when the script's directory has no dataloader.py."""
+    path = os.path.join(os.path.dirname(os.path.abspath(script)), "dataloader.py")
+    if not os.path.isfile(path):
+        return None
+    from . import trainpre
+    finder = _PatchAfterImport("dataloader", path, trainpre.install)
+    sys.meta_path.insert(0, finder)
+    return finder
+
+
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     if not argv:
@@ -276,6 +289,7 @@ def main(argv=None):
     install_shadow_modules(script)
     install_data_parallel()
     install_evaluator_patch(script)
+    install_dataloader_patch(script)
     from . import optim
     optim.install()      # torch.optim.SGD / nn.utils.clip_grad_norm_ take the flat path after a captured `_loss` (torch's otherwise)
     sys.argv = argv

@@ -439,6 +439,29 @@ int fsb_supernet_latency_bwd(const int32_t* plan_host, const int32_t* plan, cons
                              float* dalpha1, float* dalpha2, float* dbeta1, float* dbeta2, float* dratio0, float* dratio1, float* dratio2,
                              void* stream);
 
+/* --- training augmentation ------------------------------------------------------------------ */
+/* Batch geometry of fsb_train_pre: the crop (config.image_height x image_width) and the label map it is resized to
+ * (image_height / gt_down_sampling x image_width / gt_down_sampling, train/dataloader.py:25). */
+typedef struct fsb_train_pre_desc {
+  int32_t n;        /* images */
+  int32_t crop_h, crop_w;
+  int32_t label_h, label_w; /* 1 <= label_h <= crop_h, 1 <= label_w <= crop_w */
+} fsb_train_pre_desc;
+
+/* TrainPre.__call__ (train/dataloader.py:14-31, same in search/dataloader.py) for a batch, after the host drew its random numbers.
+ * img: uint8 HWC RGB sources (the dataset's img[:, :, ::-1]) and gt: uint8 HW labels, packed back to back; geom: int32 [n][8]
+ * = {H, W, mirror, sh, sw, pos_h, pos_w, pixel offset of image i in img (x3 bytes) and gt}, with 0 <= pos_h < sh,
+ * 0 <= pos_w < sw; lut: float [3][256] normalisation table.  Writes
+ *   out_img float [n][3][crop_h][crop_w]: random_mirror (tools/utils/img_utils.py:125-130), the cv2.resize INTER_LINEAR of
+ *     random_scale (:105-112), normalize (:179-184) as lut[c][v], random_crop_pad_to_shape (:24-39, pad_image_to_shape :60-74)
+ *     with 0 in the padding;
+ *   out_gt int64 [n][label_h][label_w]: the label mirrored, INTER_NEAREST resized to (sh, sw), cropped and padded with 255, then
+ *     INTER_NEAREST resized to (label_h, label_w) (train/dataloader.py:25).
+ * The resizes reproduce OpenCV's 8-bit integer arithmetic (fasterseg_b200/csrc/trainpre.cu), so with lut built from the same
+ * float64 expression as normalize, both outputs are bit-identical to the reference's tensors. */
+int fsb_train_pre(const fsb_train_pre_desc* desc, const uint8_t* img, const uint8_t* gt, const int32_t* geom, const float* lut,
+                  float* out_img, int64_t* out_gt, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

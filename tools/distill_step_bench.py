@@ -21,7 +21,9 @@ from bench import synth_weights_  # noqa: E402
 from fasterseg_b200 import zoo  # noqa: E402
 
 
-def measure(batch=12, hw=(512, 1024), steps=5, warmup=2, lazy=True, criterion="ohem"):
+def measure(batch=12, hw=(512, 1024), steps=5, warmup=2, lazy=True, criterion="ohem", data=None):
+    """data: optional callable -> (x, t) on the GPU, called once per step (a loader feeding the step); the fixed synthetic batch
+    otherwise"""
     from fasterseg_b200.losses import ProbOhemCrossEntropy2d
     B, (H, W) = batch, hw
     teacher = zoo.build_network(0).cuda().eval()
@@ -42,6 +44,9 @@ def measure(batch=12, hw=(512, 1024), steps=5, warmup=2, lazy=True, criterion="o
     t[torch.rand(t.shape, device="cuda") < 0.05] = 255
 
     def step():
+        nonlocal x, t
+        if data is not None:
+            x, t = data()
         opt.zero_grad()
         with torch.no_grad():
             tl = teacher(x).float()   # LazyLogits.float() is the identity
