@@ -20,6 +20,11 @@ int conv_wgrad_launch(const fsb_conv_desc*, const void*, const void*, int, float
 int dp_world();                                        // dp.cu: 1 unless fsb_dp_init created a communicator
 int dp_allreduce_f32(float*, int64_t, cudaStream_t);   // in-place sum over ranks on the stream
 
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+// what the vectorised BatchNorm kernels of the unit need: whole 8-channel vectors, 16-byte aligned pixels.  Checked before the
+// first launch so that a rejected call has changed nothing (the forward updates the running statistics half way through).
+static inline bool vec_view_ok(int C, int cstride, const void* p) { return C % 8 == 0 && cstride % 8 == 0 && aligned16(p); }
+
 // dgamma = sum(dz * xhat) / gscale, dbeta = sum(dz) / gscale from the rank-LOCAL sums (the data-parallel gradient average
 // divides by the world size afterwards, so these must not come from the all-reduced buffer)
 __global__ void local_param_grads_kernel(int C, const float* __restrict__ sums, float inv_gscale, float* __restrict__ dgamma,
@@ -52,8 +57,10 @@ int fsb_conv_bn_act_train_fwd(const fsb_conv_desc* d, const void* x, const void*
                               const fsb_bn_sel* sel, const int* width_idx, void* stream) {
   if (!d || !x || !wpacked || !raw_f32 || !y || !vec) return set_error(FSB_ERR_INVALID, "conv_bn_act_train_fwd: null argument");
   if ((sel == nullptr) != (width_idx == nullptr)) return set_error(FSB_ERR_INVALID, "conv_bn_act_train_fwd: sel and width_idx go together");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int C = d->Cout;
+  if (!vec_view_ok(C, raw_cstride, raw_f32) || !vec_view_ok(C, y_cstride, y) || !aligned16(vec))
+    return set_error(FSB_ERR_INVALID, "conv_bn_act_train_fwd: Cout and strides multiples of 8, raw / y / vec 16-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
   fsb_conv_desc c = *d;
   c.y_cstride = raw_cstride;
   c.flags = (d->flags & FSB_CONV_FORCE_DIRECT) | FSB_CONV_OUT_F32 | FSB_CONV_STATS;
@@ -97,6 +104,12 @@ int fsb_conv_bn_act_train_bwd(const fsb_conv_desc* d, const void* x, const void*
   const int64_t pixels = static_cast<int64_t>(d->N) * d->Ho * d->Wo;
   cudaError_t e;
   if ((sel == nullptr) != (width_idx == nullptr)) return set_error(FSB_ERR_INVALID, "conv_bn_act_train_bwd: sel and width_idx go together");
+  if (!vec_view_ok(C, dy_cstride, dy) || !vec_view_ok(C, raw_cstride, raw_f32) || !vec_view_ok(C, draw_cstride, draw) ||
+      (relu && (!y || !vec_view_ok(C, y_cstride, y))) || C > 2048)
+    return set_error(FSB_ERR_INVALID, "conv_bn_act_train_bwd: Cout <= 2048 and strides multiples of 8, dy / y / raw / draw 16-byte aligned");
+  if (dw && !x) return set_error(FSB_ERR_INVALID, "conv_bn_act_train_bwd: wgrad needs x");
+  // the dgrad's direct fallback reads the fp32 master weight; which path runs is decided inside conv_dgrad_launch
+  if (dx && (!w || dx_cstride < d->Cin)) return set_error(FSB_ERR_INVALID, "conv_bn_act_train_bwd: dx needs w and dx_cstride >= Cin");
   const int Rb = stat_rows(pixels);
   float* dgamma = vec_bwd + static_cast<size_t>(2 + 2 * Rb) * C;  // [totals (2C) | Rb partial rows | dgamma | dbeta]
   float* dbeta = dgamma + C;
@@ -124,7 +137,6 @@ int fsb_conv_bn_act_train_bwd(const fsb_conv_desc* d, const void* x, const void*
     if (rc) return rc;
   }
   if (dw) {
-    if (!x) return set_error(FSB_ERR_INVALID, "conv_bn_act_train_bwd: wgrad needs x");
     rc = conv_wgrad_launch(d, x, draw, draw_cstride, dw, so, si, 1, gscale, st);
     if (rc) return rc;
   }

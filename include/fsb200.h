@@ -327,6 +327,11 @@ int fsb_wsum_bwd(int K, int64_t pixels, int C, const void* dout, int dout_cstrid
  * backward = fsb_bn_bwd_reduce -> fsb_bn_bwd_apply -> fsb_conv_dgrad (if dx) -> fsb_conv_wgrad accumulate (if dw).
  *            vec_bwd: fp32[(4 + 2*Rb) * Cout], Rb = fsb_stat_rows(N*Ho*Wo) =
  *            [sum dz | sum dz*xhat | Rb partial rows | dgamma | dbeta]; draw: fp16 NHWC scratch.  Nothing needs zeroing.
+ * Both calls need Cout, raw_cstride and y_cstride (backward also dy_cstride, draw_cstride; Cout <= 2048) multiples of 8 and
+ *            raw / y / vec (backward dy / y / raw / draw) 16-byte aligned; the backward also needs x when dw is given, and w
+ *            and dx_cstride >= Cin when dx is given.  These arguments are checked before the first launch: a call rejected
+ *            for them returns FSB_ERR_INVALID with the running statistics, num_batches_tracked and the selected set's
+ *            gradients untouched.
  * sel / width_idx (may be NULL): the BatchNorm parameter set is chosen on the device, sel[*width_idx] (see fsb_bn_sel);
  *            gamma / beta / running stats arguments are then ignored and dgamma / dbeta accumulate into the selected set.
  * Data parallel: once fsb_dp_init() has created a communicator, both calls all-reduce their 2*Cout statistics over the ranks

@@ -381,6 +381,8 @@ WGRAD_CASES = [
     (3, 80, 160, 1, 1, 6, 10),
     (2, 32, 64, 3, 2, 9, 13),
     (1, 384, 384, 3, 1, 8, 16),
+    # FactorizedReduce's second conv: 1x1 stride 2 on x[:, :, 1:, 1:] (operations.py:523) through desc.off_h / off_w
+    (2, 64, 48, 1, 2, 12, 16, (1, 1)),
 ]
 
 
@@ -389,27 +391,28 @@ def test_conv_wgrad_and_dgrad_match_oracle(case):
     """K7: tensor-core weight gradient (MN-major operands) and data gradient vs CPU autograd of F.conv2d; the CUDA-core
     kernels are checked on the same inputs."""
     F_ = _F()
-    N, Cin, Cout, k, stride, Hh, Ww = case
+    N, Cin, Cout, k, stride, Hh, Ww = case[:7]
+    off = case[7] if len(case) > 7 else (0, 0)
     seed = hash(case) % 100000
     pad = 1 if k == 3 else 0
     x = _rand((N, Cin, Hh, Ww), seed).half().float().requires_grad_(True)
     w = (_rand((Cout, Cin, k, k), seed + 1) * (2.0 / (Cin * k * k)) ** 0.5).half().float().requires_grad_(True)
-    y = orc.conv2d(x, w, None, stride, pad)
+    y = orc.conv2d(x[:, :, off[0]:, off[1]:], w, None, stride, pad)
     gy = _rand(tuple(y.shape), seed + 2).half().float()
     y.backward(gy)
     xg, gyg, wg = _nhwc(x.detach()), _nhwc(gy), w.detach().cuda()
     for direct in (False, True):
-        dw = F_.conv_wgrad(xg, gyg, wg, Cin, Cout, k, stride, pad, 1.0, force_direct=direct)
+        dw = F_.conv_wgrad(xg, gyg, wg, Cin, Cout, k, stride, pad, 1.0, off=off, force_direct=direct)
         torch.cuda.synchronize()
         err = H.rel_err(dw.cpu().numpy(), w.grad.numpy())
         assert err < 1e-3, "wgrad (direct=%s) rel err %.3e" % (direct, err)
         wt = F_.pack_conv_weight_dgrad(wg, Cin, Cout, k)
-        dx = F_.conv_dgrad(gyg, wg, (N, Cin, Hh, Ww), Cin, Cout, k, stride, pad, wpacked_t=wt, force_direct=direct)
+        dx = F_.conv_dgrad(gyg, wg, (N, Cin, Hh, Ww), Cin, Cout, k, stride, pad, off=off, wpacked_t=wt, force_direct=direct)
         torch.cuda.synchronize()
         errx = H.rel_err(dx.float().cpu().numpy(), x.grad.numpy())
         assert errx < 1.5e-3, "dgrad (direct=%s) rel err %.3e" % (direct, errx)
     # accumulation into an existing gradient (a cell invoked twice, model_search.py:326-329)
     acc = dw.clone()
-    F_.conv_wgrad(xg, gyg, wg, Cin, Cout, k, stride, pad, 1.0, accumulate_into=acc)
+    F_.conv_wgrad(xg, gyg, wg, Cin, Cout, k, stride, pad, 1.0, off=off, accumulate_into=acc)
     torch.cuda.synchronize()
     assert H.rel_err(acc.cpu().numpy(), 2 * w.grad.numpy()) < 1e-3
