@@ -121,7 +121,8 @@ int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, 
 int conv_tc_occupancy(const ConvPlan& plan);
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride);
 int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
-                         float gscale, cudaStream_t stream);
+                         int accumulate, float gscale, cudaStream_t stream);
+int zero_wgrad_launch(const fsb_conv_desc* d, float* dw, int64_t so, int64_t si, cudaStream_t stream);
 int conv_direct_launch(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
                        void* y, float* stats, cudaStream_t stream);
 

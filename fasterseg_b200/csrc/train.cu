@@ -373,16 +373,20 @@ __global__ void __launch_bounds__(128) conv_dgrad_direct_kernel(const DgradParam
     if (cg * 8 + j < d.Cin) xp[j] = __float2half_rn(acc[j]);
 }
 
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 int conv_dgrad_launch(const fsb_conv_desc* d, const void* dy, int dcs, const void* wpacked_t, const float* w, int64_t so,
                       int64_t si, void* dx, int xcs, cudaStream_t stream) {
-  if (d->stride == 1 && d->off_h == 0 && d->off_w == 0 && wpacked_t && !(d->flags & FSB_CONV_FORCE_DIRECT)) {
+  // the tensor-core paths read dy and the packed weight through TMA (16-byte aligned bases); anything else takes the direct kernel
+  const bool tc_ok = wpacked_t && aligned16(wpacked_t) && aligned16(dy) && !(d->flags & FSB_CONV_FORCE_DIRECT);
+  if (d->stride == 1 && d->off_h == 0 && d->off_w == 0 && tc_ok) {
     fsb_conv_desc t = dgrad_as_fwd_desc(d, dcs, xcs);
     if (conv_tc_supported(&t)) return conv_tc_launch(conv_plan(&t, nullptr, false), &t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream);
   }
   // stride 2: the input pixels of each (row, column) parity receive contributions from a fixed subset of filter taps; each
   // parity plane is a stride-1 implicit GEMM over dy with that tap subset, written to the plane through a strided tensor map
-  if (d->stride == 2 && wpacked_t && !(d->flags & FSB_CONV_FORCE_DIRECT) && d->Cin % 8 == 0 && xcs % 8 == 0 && dcs % 8 == 0 &&
-      d->Cout >= 16 && (reinterpret_cast<uintptr_t>(dx) & 15) == 0 && opt(OPT_DGRAD_S2_DIRECT) <= 0) {
+  if (d->stride == 2 && tc_ok && d->Cin % 8 == 0 && xcs % 8 == 0 && dcs % 8 == 0 && d->Cout >= 16 && aligned16(dx) &&
+      opt(OPT_DGRAD_S2_DIRECT) <= 0) {
     fsb_conv_desc t = dgrad_as_fwd_desc(d, dcs, xcs);  // stride-1 problem over dy; geometry fields only feed the packer
     t.pad = 0;
     t.Ho = d->Ho;
@@ -421,14 +425,23 @@ int conv_dgrad_launch(const fsb_conv_desc* d, const void* dy, int dcs, const voi
         c.y_strides[1] = 2ull * d->W * xcs * 2;
         c.y_strides[2] = static_cast<uint64_t>(d->H) * d->W * xcs * 2;
       }
-    if (need_zero) {
-      cudaError_t e = cudaMemsetAsync(dx, 0, static_cast<size_t>(d->N) * d->H * d->W * xcs * 2, stream);
-      if (e != cudaSuccess) return set_cuda_error(e, "conv_dgrad: memset");
-    }
     if (conv_tc_supported(&t)) {
+      ConvPlan plans[4];
+      for (int i = 0; i < 4; ++i) {  // descriptor errors before the first write
+        if (!live[i]) continue;
+        plans[i] = conv_plan(&t, &planes[i]);
+        if (plans[i].rc) return plans[i].rc;
+      }
+      // a parity plane without taps (1x1 stride 2) gets no MMA: zero the Cin channels of every pixel, not the whole pixel
+      // stride, which belongs to the caller when dx is a channel slice
+      if (need_zero) {
+        cudaError_t e = cudaMemset2DAsync(dx, static_cast<size_t>(xcs) * 2, 0, static_cast<size_t>(d->Cin) * 2,
+                                          static_cast<size_t>(d->N) * d->H * d->W, stream);
+        if (e != cudaSuccess) return set_cuda_error(e, "conv_dgrad: memset");
+      }
       for (int i = 0; i < 4; ++i) {
         if (!live[i]) continue;
-        int rc = conv_tc_launch(conv_plan(&t, &planes[i]), &t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream, &planes[i]);
+        int rc = conv_tc_launch(plans[i], &t, dy, wpacked_t, nullptr, nullptr, dx, nullptr, stream, &planes[i]);
         if (rc) return rc;
       }
       return FSB_OK;
@@ -549,17 +562,24 @@ __global__ void zero_wgrad_kernel(float* dw, int64_t so, int64_t si, int Cout, i
     dw[co * so + ci * si + t] = 0.f;
   }
 }
+// zeroes the [0,Cout) x [0,Cin) corner of the gradient before an accumulate = 0 weight gradient
+int zero_wgrad_launch(const fsb_conv_desc* d, float* dw, int64_t so, int64_t si, cudaStream_t stream) {
+  const int taps = d->ksize * d->ksize;
+  const int64_t total = static_cast<int64_t>(d->Cout) * d->Cin * taps;
+  FSB_LAUNCH(zero_wgrad_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream, dw, so, si, d->Cout, d->Cin, taps);
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "zero_wgrad launch");
+  return FSB_OK;
+}
 int conv_wgrad_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
                       int accumulate, float gscale, cudaStream_t stream) {
   const int taps = d->ksize * d->ksize;
-  if (!accumulate) {
-    const int64_t total = static_cast<int64_t>(d->Cout) * d->Cin * taps;
-    FSB_LAUNCH(zero_wgrad_kernel, dim3(grid_for(total, 256)), dim3(256), 0, stream, dw, so, si, d->Cout, d->Cin, taps);
-    cudaError_t e0 = last_launch_error();
-    if (e0 != cudaSuccess) return set_cuda_error(e0, "zero_wgrad launch");
-  }
-  if (conv_wgrad_tc_supported(d, dcs) && !(d->flags & FSB_CONV_FORCE_DIRECT))
-    return conv_wgrad_tc_launch(d, x, dy, dcs, dw, so, si, gscale, stream);
+  // the tensor-core kernel reads x and dy through TMA (16-byte aligned bases); the direct kernel has no alignment needs.  The
+  // tensor-core launch zeroes dw itself, once its tensor maps are encoded, so that a call it rejects writes nothing.
+  if (conv_wgrad_tc_supported(d, dcs) && aligned16(x) && aligned16(dy) && !(d->flags & FSB_CONV_FORCE_DIRECT))
+    return conv_wgrad_tc_launch(d, x, dy, dcs, dw, so, si, accumulate, gscale, stream);
+  if (!accumulate)
+    if (int rc = zero_wgrad_launch(d, dw, so, si, stream)) return rc;
   WgradParams p;
   p.d = *d;
   p.x = static_cast<const __half*>(x);

@@ -157,11 +157,18 @@ int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride) {
   if (!(d->ksize == 1 || d->ksize == 3) || !(d->stride == 1 || d->stride == 2) || d->dil != 1) return 0;
   if (d->Cin < 16 || d->Cout < 16 || (d->x_cstride % 8) != 0 || (dy_cstride % 8) != 0) return 0;
   if (opt(OPT_WGRAD_TC) == 0) return 0;
+  // stride 2 reads each tap from a parity plane of x: a 1-pixel-high or -wide input may leave a tap's plane empty
+  if (d->stride == 2)
+    for (int r = 0; r < d->ksize; ++r)
+      for (int s = 0; s < d->ksize; ++s) {
+        const int ph = (((r - d->pad + d->off_h) % 2) + 2) % 2, pw = (((s - d->pad + d->off_w) % 2) + 2) % 2;
+        if ((d->H - ph + 1) / 2 <= 0 || (d->W - pw + 1) / 2 <= 0) return 0;
+      }
   return 1;
 }
 
 int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, int dcs, float* dw, int64_t so, int64_t si,
-                         float gscale, cudaStream_t stream) {
+                         int accumulate, float gscale, cudaStream_t stream) {
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(dy) & 15))
     return set_error(FSB_ERR_INVALID, "wgrad_tc: x / dy must be 16-byte aligned");
   WgradTcParams p;
@@ -253,6 +260,8 @@ int conv_wgrad_tc_launch(const fsb_conv_desc* d, const void* x, const void* dy, 
   const void* kernel = ci_tile == 128 ? reinterpret_cast<const void*>(conv_wgrad_tc_kernel<128>)
                                       : reinterpret_cast<const void*>(conv_wgrad_tc_kernel<64>);
   if (int rc = ensure_dyn_smem(kernel, 220 * 1024, "cudaFuncSetAttribute(conv_wgrad_tc)")) return rc;
+  if (!accumulate)  // only now: every check above returns before anything is written
+    if (int rc = zero_wgrad_launch(d, dw, so, si, stream)) return rc;
   dim3 grid(static_cast<unsigned>(fixed), static_cast<unsigned>(chunks));
   const cudaError_t e = ci_tile == 128 ? launch_kernel(conv_wgrad_tc_kernel<128>, grid, dim3(kWgThreads), smem_bytes, stream, p)
                                        : launch_kernel(conv_wgrad_tc_kernel<64>, grid, dim3(kWgThreads), smem_bytes, stream, p);

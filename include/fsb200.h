@@ -285,8 +285,17 @@ int fsb_relu_bwd(int64_t pixels, int C, const void* dy, int dy_cstride, const vo
 /* conv data gradient (autograd of F.conv2d wrt input): dx[n,hi,wi,ci] = sum_{r,s,co} dy[n,ho,wo,co] * w[co,ci,r,s] over the
  * (ho,wo,r,s) with ho*stride + r - pad + off_h == hi (same for w).  `d` describes the FORWARD conv (x: N,H,W,Cin ...);
  * dy has d->Ho x d->Wo x Cout with pixel stride dy_cstride; dx has H x W x Cin with pixel stride dx_cstride.
- * w: fp32 OIHW master weight with strides like fsb_pack_conv_weight.  Stride-1 convs run on the tensor-core kernel with
- * a transposed/rotated weight pack (wpacked_t from fsb_pack_conv_weight_dgrad); others use the direct kernel. */
+ * w: fp32 OIHW master weight with strides like fsb_pack_conv_weight.  Paths, given wpacked_t (the transposed / rotated pack of
+ * fsb_pack_conv_weight_dgrad), a 16-byte aligned dy and wpacked_t, and no FSB_CONV_FORCE_DIRECT:
+ *   - stride 1 without an input offset: the tensor-core conv kernel (Cout >= 16, dy_cstride % 8 == 0), per-tap or window mode;
+ *   - stride 2: one stride-1 tensor-core GEMM per (row, column) parity plane of dx (Cout >= 16; Cin, dx_cstride and dy_cstride
+ *     multiples of 8; dx 16-byte aligned; FSB_DGRAD_S2_DIRECT=1 turns it off).  A plane that no filter tap reaches (1x1
+ *     stride 2) is zeroed: only its Cin channels, so dx may be a channel slice of a wider buffer;
+ *   - everything else, misaligned dy included: the direct CUDA-core kernel, which needs w (FSB_ERR_INVALID before any write
+ *     without it).
+ * Every dx element of the Cin channels is written; the channels beyond Cin in the pixel stride are never touched.  Argument
+ * and descriptor errors return before any write; only a failure to encode a TMA tensor map or to launch (a CUDA error) can
+ * follow the stride-2 zeroing. */
 size_t fsb_conv_packed_dgrad_bytes(const fsb_conv_desc* d);
 int fsb_pack_conv_weight_dgrad(const fsb_conv_desc* d, const float* w, int64_t w_stride_o, int64_t w_stride_i, void* packed_t,
                                void* stream);
@@ -294,7 +303,13 @@ int fsb_conv_dgrad(const fsb_conv_desc* d, const void* dy, int dy_cstride, const
                    int64_t w_stride_o, int64_t w_stride_i, void* dx, int dx_cstride, void* stream);
 /* conv weight gradient: dw[co,ci,r,s] (+)= (1/gscale) * sum_{n,ho,wo} dy[n,ho,wo,co] * x[n, ho*stride+r-pad+off_h, ..., ci]
  * written into the fp32 OIHW gradient tensor with the master weight's strides (only the [0,Cout) x [0,Cin) corner).
- * accumulate != 0 adds to the existing contents (a cell invoked twice, model_search.py:326-329). */
+ * accumulate != 0 adds to the existing contents (a cell invoked twice, model_search.py:326-329); accumulate == 0 zeroes the
+ * corner first.  Elements outside the corner are never touched.  1x1 / 3x3, stride 1 or 2, dilation 1, Cin, Cout >= 16,
+ * x_cstride and dy_cstride multiples of 8, 16-byte aligned x and dy, no stride-2 parity plane of x left empty (H or W of 1),
+ * no FSB_CONV_FORCE_DIRECT and FSB_WGRAD_TC != 0: the tensor-core kernel; everything else (misaligned x or dy included) the
+ * direct CUDA-core kernel.  Every rejection (FSB_ERR_INVALID, or a TMA tensor map that cannot be encoded) returns before dw is
+ * zeroed or written.  Both kernels split the pixels over CTAs that add with fp32 atomics, except under FSB_DETERMINISTIC=1,
+ * where each element has one writer and the result is bit-reproducible. */
 int fsb_conv_wgrad(const fsb_conv_desc* d, const void* x, const void* dy, int dy_cstride, float* dw, int64_t w_stride_o,
                    int64_t w_stride_i, int accumulate, float gscale, void* stream);
 
