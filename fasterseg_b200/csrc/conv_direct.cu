@@ -126,8 +126,7 @@ int conv_direct_launch(const fsb_conv_desc* d, const void* x, const void* wpacke
   FSB_LAUNCH(conv_direct_kernel, dim3(static_cast<unsigned>(blocks)), dim3(128), 0, stream, p);
   cudaError_t e = last_launch_error();
   if (e != cudaSuccess) return set_cuda_error(e, "conv_direct launch");
-  if (want_stats) {
-    if (d->flags & (FSB_CONV_AFFINE | FSB_CONV_RELU)) return set_error(FSB_ERR_INVALID, "conv_direct: STATS needs a raw (no epilogue) output");
+  if (want_stats) {  // conv_plan admits FSB_CONV_STATS only with a raw fp32 output
     const int SC = d->stats_C > 0 ? d->stats_C : d->Cout;
     return bn_stats_rows_launch(static_cast<int64_t>(d->N) * d->Ho * d->Wo, d->Cout, y, d->y_cstride,
                                 (d->flags & FSB_CONV_OUT_F32) ? 1 : 0, stats + d->stats_off, SC, stream);

@@ -486,8 +486,26 @@ int conv_tc_supported(const fsb_conv_desc* d) {
 // static shared memory of an instance: the 2 * kMaxStages + 4 mbarriers and s_scale / s_shift of conv_tc_body
 static size_t conv_tc_static_smem(int n_tile) { return (2 * kMaxStages + 4) * 8 + static_cast<size_t>(n_tile) * 2 * 4; }
 
-// descriptor checks of conv_plan: the flag combinations no kernel runs
+// a stride-2 tap reads a parity plane of x without pixels (H or W of 1): no tensor map can address it, the direct kernel runs it
+static bool conv_tc_empty_plane(const fsb_conv_desc* d) {
+  if (d->stride != 2) return false;
+  for (int r = 0; r < d->ksize; ++r)
+    for (int s = 0; s < d->ksize; ++s) {
+      const int qh = r * d->dil - d->pad + d->off_h, qw = s * d->dil - d->pad + d->off_w;
+      const int ph = ((qh % 2) + 2) % 2, pw = ((qw % 2) + 2) % 2;
+      if ((d->H - ph + 1) / 2 <= 0 || (d->W - pw + 1) / 2 <= 0) return true;
+    }
+  return false;
+}
+
+// descriptor checks of conv_plan: the flag combinations no kernel runs.  Every path rejects them before any launch.
 static int conv_check_flags(const fsb_conv_desc* d, bool direct, const ConvTcCustom* cu) {
+  // the statistics are those of the raw fp32 conv output: the direct kernel takes them from the stored output, so it must be
+  // that value (no epilogue, fp32), and conv_tc returns the same for the same descriptor
+  if ((d->flags & FSB_CONV_STATS) && ((d->flags & (FSB_CONV_AFFINE | FSB_CONV_RELU)) || !(d->flags & FSB_CONV_OUT_F32)))
+    return set_error(FSB_ERR_INVALID, "conv_fwd: FSB_CONV_STATS needs FSB_CONV_OUT_F32 and no FSB_CONV_AFFINE / FSB_CONV_RELU");
+  if ((d->flags & FSB_CONV_STATS) && (d->stats_off < 0 || d->stats_off + d->Cout > (d->stats_C > 0 ? d->stats_C : d->Cout)))
+    return set_error(FSB_ERR_INVALID, "conv_fwd: stats_off + Cout exceeds stats_C");
   if (direct && (d->flags & (FSB_CONV_X_DOWN2 | FSB_CONV_Y_UP2)))
     return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd: FSB_CONV_X_DOWN2 / FSB_CONV_Y_UP2 need the wgmma kernel (Cin >= 16, x_cstride % 8 == 0, "
                                           "no FSB_CONV_FORCE_DIRECT)");
@@ -504,7 +522,7 @@ static int conv_check_flags(const fsb_conv_desc* d, bool direct, const ConvTcCus
 
 ConvPlan conv_plan(const fsb_conv_desc* d, const ConvTcCustom* cu, bool window_ok) {
   ConvPlan pl = {};
-  pl.direct = (d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d);
+  pl.direct = (d->flags & FSB_CONV_FORCE_DIRECT) || !conv_tc_supported(d) || (!cu && conv_tc_empty_plane(d));
   pl.rc = conv_check_flags(d, pl.direct, cu);
   if (pl.direct) {
     pl.stat_rows = stat_rows(static_cast<int64_t>(d->N) * d->Ho * d->Wo);
@@ -660,8 +678,6 @@ int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, 
   p.stats = stats;
   p.stats_C = d->stats_C > 0 ? d->stats_C : d->Cout;
   p.stats_off = d->stats_off;
-  if ((d->flags & FSB_CONV_STATS) && stats && (d->stats_off < 0 || d->stats_off + d->Cout > p.stats_C))
-    return set_error(FSB_ERR_INVALID, "conv_tc: stats_off + Cout exceeds stats_C");
   // ---- TMA-store epilogue: fp16 output whose pixels start on 16 B and whose channel count is a multiple of 8 ----
   // FSB_CONV_Y_UP2: y is the 2Ho x 2Wo map and every output pixel goes to its 2x2 block (nearest x2 folded into the store):
   // four lattice maps, one per (row, column) parity, each with the pixel steps of the full map doubled; the epilogue stores
@@ -750,7 +766,7 @@ int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, 
       for (int pw = 0; pw < 2; ++pw) {
         if (!used[ph * 2 + pw]) continue;
         const int Hp = (d->H - ph + 1) / 2, Wp = (d->W - pw + 1) / 2;
-        if (Hp <= 0 || Wp <= 0) return set_error(FSB_ERR_INVALID, "conv_tc: empty parity plane");
+        if (Hp <= 0 || Wp <= 0) return set_error(FSB_ERR_INVALID, "conv_tc: empty parity plane");  // conv_plan routes these to direct
         const uint64_t dims[4] = {static_cast<uint64_t>(d->Cin), static_cast<uint64_t>(Wp), static_cast<uint64_t>(Hp),
                                   static_cast<uint64_t>(d->N)};
         const uint64_t str[3] = {2 * cs, 2 * cs * d->W, cs * d->W * d->H};

@@ -44,8 +44,10 @@ typedef enum fsb_status {
 #define FSB_CONV_OUT_F32 16u    /* y is fp32 NHWC (y_cstride in fp32 elements): the training path keeps the raw conv output in
                                    fp32 so that BatchNorm normalises un-rounded values, like the fp32 reference */
 #define FSB_ACT_IN_F32 32u      /* fsb_affine_act: x is fp32 NHWC */
-#define FSB_CONV_STATS 8u       /* also produce per-channel sum / sum-of-squares of the (pre-affine) fp32 conv output as
-                                   PARTIAL ROWS, one per CTA (BN train, K2) -- see "Deterministic statistics" below */
+#define FSB_CONV_STATS 8u       /* also produce per-channel sum / sum-of-squares of the fp32 conv output as PARTIAL ROWS, one
+                                   per CTA (BN train, K2) -- see "Deterministic statistics" below.  Only with FSB_CONV_OUT_F32
+                                   and without FSB_CONV_AFFINE / FSB_CONV_RELU (the raw output is what is summed, on every
+                                   kernel); any other combination is FSB_ERR_INVALID before anything is written */
 /* Nearest-neighbour resizes folded into the tensor maps of the wgmma conv (latency/ deployment network,
  * latency/operations.py:265,269,427,434, latency/model_seg.py:305,309,315).  Addresses change, nothing else: the result is
  * bit for bit the conv of the resized input / the resized conv output. */
@@ -135,9 +137,13 @@ int fsb_bn_fold(int C, const float* gamma, const float* beta, const float* mean,
 /* y[n,ho,wo,co] = act( (sum_{r,s,ci} x[n, ho*stride + r*dil - pad + off_h, wo*stride + s*dil - pad + off_w, ci]
  *                      * w[co,ci,r,s]) * scale[co] + shift[co] )
  * x, y: fp16 NHWC with the strides in `d`; wpacked from fsb_pack_conv_weight; scale/shift fp32[Cout] or NULL;
- * stats fp32[2*Cout] (only with FSB_CONV_STATS; caller zeroes it).
+ * stats: fp32[fsb_conv_stats_rows(d) * 2 * SC] partial rows (only with FSB_CONV_STATS; no zeroing needed).
  * Dense 3x3 / 1x1 contractions run as an im2col-free implicit GEMM on the wgmma tensor cores with TMA-staged
- * NHWC tiles; Cin < 16 (the RGB stem) and FSB_CONV_FORCE_DIRECT use the CUDA-core direct kernel. */
+ * NHWC tiles; Cin < 16 (the RGB stem), x_cstride % 8 != 0, a stride-2 conv one of whose taps reads no input row or column
+ * (H or W of 1) and FSB_CONV_FORCE_DIRECT use the CUDA-core direct kernel.  The choice is made from the descriptor alone
+ * (fsb_conv_kernel_id, fsb_conv_stats_rows): a descriptor the wgmma kernel takes whose x or wpacked is not 16-byte aligned
+ * (TMA) is FSB_ERR_INVALID, before anything is written -- it does not fall back to the direct kernel, whose statistics rows
+ * would not be the fsb_conv_stats_rows(d) the caller sized the buffer for. */
 int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
                  void* y, float* stats, void* stream);
 /* which kernel fsb_conv_fwd dispatches for `d`: 0 = CUDA-core direct, 1 = the wgmma kernel conv_tc on 16x8 / 8x16 pixel tiles

@@ -81,8 +81,32 @@ def bn_fold(gamma, beta, mean, var, eps, conv_bias=None):
 PRECISE = {"on": False}
 
 
+# shape-only convs and conv gradients: zeros of the right shape instead of the arithmetic, for recording which calls a network
+# makes where its control flow does not depend on the data (tests/conv_fwd_census.py)
+SHAPES_ONLY = {"on": False}
+
+
+@contextlib.contextmanager
+def shapes_only():
+    SHAPES_ONLY["on"] = True
+    try:
+        yield
+    finally:
+        SHAPES_ONLY["on"] = False
+
+
+def _conv2d(x, w, stride, pad):
+    if SHAPES_ONLY["on"]:
+        N, _, H, W = x.shape
+        k = w.shape[2]
+        return torch.zeros((N, w.shape[0], (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1), dtype=torch.float32)
+    return TF.conv2d(x, w, None, stride, pad)
+
+
 def _raw_conv(x, w16, stride, pad, off):
     xin = x[:, :, off[0]:, off[1]:].float()
+    if SHAPES_ONLY["on"]:
+        return _conv2d(xin, w16, stride, pad)
     if PRECISE["on"]:
         return TF.conv2d(xin.double(), w16.double(), None, stride, pad).float()
     return TF.conv2d(xin, w16.float(), None, stride, pad)
@@ -106,9 +130,13 @@ def rowsum(rows):
 
 
 def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=False, out=None, off=(0, 0),
-             stats=None, force_direct=False, out_f32=False, stats_off=0):
+             stats=None, force_direct=False, out_f32=False, stats_off=0, down2=False, up2=False):
     N, Cin, H, W, _ = nhwc_info(x)
     assert tuple(wpacked.shape) == (Cout, Cin, ksize, ksize), (tuple(wpacked.shape), (Cout, Cin, ksize, ksize))
+    if down2:      # nearest(x, (H/2, W/2)): the even rows and columns (FSB_CONV_X_DOWN2)
+        assert H % 2 == 0 and W % 2 == 0 and stride == 1 and stats is None and not out_f32
+        x = x[:, :, ::2, ::2]
+        H, W = H // 2, W // 2
     y = _raw_conv(x, wpacked, stride, pad, off)
     Ho, Wo = F_.conv_out_size(H, W, ksize, stride, pad, 1, off[0], off[1])
     assert tuple(y.shape) == (N, Cout, Ho, Wo)
@@ -120,6 +148,10 @@ def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=
         y = y + shift.view(1, -1, 1, 1)
     if relu:
         y = y.relu()
+    if up2:        # nearest(y, (2Ho, 2Wo)): every output pixel to its 2x2 block (FSB_CONV_Y_UP2)
+        assert stats is None and not out_f32
+        y = y.repeat_interleave(2, 2).repeat_interleave(2, 3)
+        Ho, Wo = 2 * Ho, 2 * Wo
     odt = torch.float32 if out_f32 else torch.float16
     if out is None:
         out = _empty(N, Cout, Ho, Wo, x.device, dtype=odt)
@@ -130,7 +162,7 @@ def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=
 
 def stem_conv_nchw(x, w, scale, shift, relu=True, out=None):
     assert x.dim() == 4 and x.shape[1] == 3 and tuple(w.shape[1:]) == (3, 3, 3)
-    y = TF.conv2d(x.half().float(), w.half().float(), None, 2, 1)
+    y = _conv2d(x.half().float(), w.half().float(), 2, 1)
     if scale is not None:
         y = y * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1)
     if relu:
@@ -143,7 +175,7 @@ def stem_conv_nchw(x, w, scale, shift, relu=True, out=None):
 def stem_conv_u8hwc(x_u8, lut, w, scale, shift, relu=True, out=None):
     N, _, H, W = x_u8.shape
     xn = torch.stack([lut.view(3, 256)[c][x_u8[:, c].long()] for c in range(3)], dim=1).float()   # fp16 table values
-    y = TF.conv2d(xn, w.half().float(), None, 2, 1)
+    y = _conv2d(xn, w.half().float(), 2, 1)
     if scale is not None:
         y = y * scale.view(1, -1, 1, 1) + shift.view(1, -1, 1, 1)
     if relu:
@@ -192,6 +224,39 @@ def upsample_logits(x, size, dtype=torch.float32, out=None):
 def upsample_argmax(x, size, out=None):
     nhwc_info(x)
     lab = _interp(x.float(), size).argmax(1).to(torch.uint8)
+    if out is not None:
+        out.copy_(lab)
+        return out
+    return lab
+
+
+def _nearest(x32, size):
+    """torch's legacy 'nearest' index rule (src = floor(dst * in / out)), as the library's nearest kernels (include/fsb200.h)"""
+    return TF.interpolate(x32, size=(int(size[0]), int(size[1])), mode="nearest")
+
+
+def nearest(x, size, out=None):
+    N, Cc, _, _, _ = nhwc_info(x)
+    y = _nearest(x.float(), size)
+    if out is None:
+        out = _empty(N, Cc, int(size[0]), int(size[1]), x.device)
+    assert tuple(out.shape) == tuple(y.shape)
+    nhwc_info(out)
+    return _put(out, y)
+
+
+def upsample_logits_nearest(x, size, dtype=torch.float32, out=None):
+    nhwc_info(x)
+    y = _nearest(x.float(), size).to(dtype).contiguous()
+    if out is not None:
+        out.copy_(y)
+        return out
+    return y
+
+
+def upsample_argmax_nearest(x, size, out=None):
+    nhwc_info(x)
+    lab = _nearest(x.float(), size).argmax(1).to(torch.uint8)
     if out is not None:
         out.copy_(lab)
         return out
@@ -278,7 +343,9 @@ def conv_dgrad(dy, w, x_shape, Cin, Cout, ksize, stride, pad, off=(0, 0), wpacke
     nhwc_info(dy)
     w16 = w[:Cout, :Cin].detach().half().float()
     eff = (N, Cin, H - off[0], W - off[1])
-    if PRECISE["on"]:
+    if SHAPES_ONLY["on"]:
+        g = torch.zeros(eff, dtype=torch.float32)
+    elif PRECISE["on"]:
         g = torch.nn.grad.conv2d_input(eff, w16.double(), dy.double(), stride=stride, padding=pad).float()
     else:
         g = torch.nn.grad.conv2d_input(eff, w16, dy.float(), stride=stride, padding=pad)
@@ -289,7 +356,9 @@ def conv_dgrad(dy, w, x_shape, Cin, Cout, ksize, stride, pad, off=(0, 0), wpacke
 
 def conv_wgrad(x, dy, w_like, Cin, Cout, ksize, stride, pad, gscale, off=(0, 0), accumulate_into=None, force_direct=False):
     xin = x[:, :, off[0]:, off[1]:].float()
-    if PRECISE["on"]:
+    if SHAPES_ONLY["on"]:
+        g = torch.zeros((Cout, Cin, ksize, ksize), dtype=torch.float32)
+    elif PRECISE["on"]:
         g = (torch.nn.grad.conv2d_weight(xin.double(), (Cout, Cin, ksize, ksize), dy.double(), stride=stride, padding=pad) / gscale).float()
     else:
         g = torch.nn.grad.conv2d_weight(xin, (Cout, Cin, ksize, ksize), dy.float(), stride=stride, padding=pad) / gscale
@@ -467,7 +536,7 @@ def conv_bn_act_train_bwd_sel(d, x, dy, y, raw, vec, sel, relu, wpacked_t, w, ne
 
 
 _PATCHED = ("nhwc_info", "to_nhwc_half", "to_nchw", "pack_conv_weight", "bn_fold", "conv_stats_buffer", "rowsum", "conv_fwd", "stem_conv_nchw", "bilinear",
-            "upsample_logits", "upsample_argmax", "copy_channels", "bn_stats", "bn_finalize", "affine_act", "bn_bwd_sums", "bn_bwd_apply", "relu_bwd",
+            "upsample_logits", "upsample_argmax", "nearest", "upsample_logits_nearest", "upsample_argmax_nearest", "copy_channels", "bn_stats", "bn_finalize", "affine_act", "bn_bwd_sums", "bn_bwd_apply", "relu_bwd",
             "pack_conv_weight_dgrad", "conv_dgrad", "conv_wgrad", "bilinear_bwd", "upsample_logits_bwd", "nchw_grad_to_nhwc",
             "wsum_fwd", "wsum_bwd", "add_inplace", "conv_bn_act_train_fwd", "conv_bn_act_train_bwd",
             "stem_conv_u8hwc", "confusion_matrix", "bn_finalize_sel", "affine_act_sel", "bn_bwd_sel", "conv_bn_act_train_fwd_sel", "conv_bn_act_train_bwd_sel",

@@ -22,32 +22,12 @@ import pytest
 import torch
 
 from tests import conv_bwd_census as CC
+from tests.conv_harness import (F64, INVALID, SENT16, SENT32, U, L, Options, Slice, _assert_kernels, _bits32, _cpad, _ints, _n_tile,
+                                _normal, _out_size, _report, _s, profiled)
 
 pytestmark = pytest.mark.gpu
 
-F64 = torch.float64
-U = 2.0 ** -24
 GSCALE = 1024.0            # autograd.GRAD_SCALE
-SENT16, SENT32 = 1000.0, -777.0
-INVALID = -1
-
-
-def L():
-    from fasterseg_b200 import _lib
-    return _lib.lib()
-
-
-def _s():
-    return torch.cuda.current_stream().cuda_stream
-
-
-def _cpad(c):
-    return (c + 7) // 8 * 8
-
-
-def _out_size(H, W, k, s, p, dil, off):
-    e = dil * (k - 1) + 1
-    return (H - off[0] + 2 * p - e) // s + 1, (W - off[1] + 2 * p - e) // s + 1
 
 
 class G:
@@ -82,27 +62,6 @@ class G:
 
 
 # ---- which path a geometry takes (mirrors the routing of conv_dgrad_launch / conv_wgrad_launch / conv_plan) ------------------------
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def _n_tile(Cout_t, Ho, Wo, N):
-    """conv_plan's output-channel tile for a conv_tc problem with Cout_t output channels on an Ho x Wo map"""
-    kNt = [16, 32, 48, 64, 96, 128]
-    npad = (Cout_t + 15) // 16 * 16
-    tw = 16 if Wo >= 16 else 8
-    m_tiles = -(-Wo // tw) * -(-Ho // (128 // tw)) * N
-    n_tiles = -(-npad // 128)
-    ni = 0
-    while kNt[ni] * n_tiles < npad:
-        ni += 1
-    n_tiles = -(-npad // kNt[ni])
-    while m_tiles * n_tiles < _sms() and ni > 0 and kNt[ni - 1] >= 32:
-        ni -= 1
-        n_tiles = -(-npad // kNt[ni])
-    return kNt[ni]
-
-
 def _s2_planes(g):
     """-> [(Hl, Wl, ntaps)] of the four parity planes of a stride-2 dgrad"""
     out = []
@@ -163,122 +122,6 @@ def dgrad_paths(g, dcs, dxcs, aligned=True):
         return [("planes", 0, {"FSB_DGRAD_S2_DIRECT": -1}, dict(exp)), ("s2_direct", 0, {"FSB_DGRAD_S2_DIRECT": 1}, direct),
                 ("direct", FD, {}, direct)]
     return [("direct", 0, {}, direct)]
-
-
-def _kernel_key(name):
-    """profiler kernel name -> the key the expectations use: conv_tc instances by (n_tile, window), the rest by name"""
-    n = name.replace("void ", "").replace("fsb::", "").split("(")[0]
-    if n.startswith("conv_tc_kernel<"):
-        bk, nt, win = [a.strip() for a in n[len("conv_tc_kernel<"):-1].split(",")]
-        return "conv_tc%s<%s>" % ("_win" if win == "true" else "", nt)
-    return n
-
-
-class Kernels:
-    """counts the library's conv backward kernel launches of a block (torch.profiler; the weight packing the dgrad runs need is
-    left out).  CUPTI hands its activity records over in buffers, and a buffer can reach the profiler after the session that
-    launched its kernels has ended, i.e. inside the next one.  So only the records of this block's own launches count: the
-    kernels whose CUPTI correlation id belongs to a launch call made inside the block's time range.  `stale` counts the
-    records of earlier launches that arrived here."""
-    NAME = "conv_bwd_kernels"
-
-    def __enter__(self):
-        from torch.profiler import ProfilerActivity, profile, record_function
-        torch.cuda.synchronize()
-        self.prof = profile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA])
-        self.prof.__enter__()
-        self.mark = record_function(self.NAME)
-        self.mark.__enter__()
-        return self
-
-    def __exit__(self, *exc):
-        torch.cuda.synchronize()
-        self.mark.__exit__(*exc)
-        self.prof.__exit__(*exc)
-        CUDA = torch.autograd.DeviceType.CUDA
-        evs = list(self.prof.profiler.kineto_results.events())
-        mark = [e for e in evs if e.name() == self.NAME and e.device_type() != CUDA]
-        assert len(mark) == 1, "the block's annotation is missing from the trace"
-        t0, t1 = mark[0].start_ns(), mark[0].end_ns()
-        own = {e.correlation_id() for e in evs
-               if e.device_type() != CUDA and e.name().startswith("cudaLaunchKernel") and t0 <= e.start_ns() <= t1}
-        # the library launches through cudaLaunchKernelEx (cudaLaunchKernelExC in the trace): each of those launches of the
-        # block must have its kernel record, none still in a CUPTI buffer
-        lib = {e.correlation_id() for e in evs
-               if e.device_type() != CUDA and e.name().startswith("cudaLaunchKernelExC") and t0 <= e.start_ns() <= t1}
-        self.complete = lib <= {e.correlation_id() for e in evs if e.device_type() == CUDA}
-        kernels = [e for e in evs if e.device_type() == CUDA and "fsb::" in e.name()]
-        self.stale = sum(1 for e in kernels if e.correlation_id() not in own)
-        self.counts = collections.Counter(_kernel_key(e.name()) for e in kernels
-                                          if e.correlation_id() in own and "pack_dgrad_kernel" not in e.name())
-
-
-def profiled(fn):
-    """-> (fn(), Kernels of its launches).  A trace in which a launch of the block has no kernel record yet is incomplete: the
-    block (fresh buffers, same inputs) is run again, at most three times in all."""
-    for _ in range(3):
-        with Kernels() as k:
-            out = fn()
-        if k.complete:
-            return out, k
-    raise AssertionError("the profiler's trace missed launches of the block three times")
-
-
-class Options:
-    def __init__(self, opts):
-        self.opts = opts
-
-    def __enter__(self):
-        from fasterseg_b200 import _lib
-        self.saved = {k: _lib.get_option(k) for k in self.opts}
-        for k, v in self.opts.items():
-            _lib.set_option(k, v)
-
-    def __exit__(self, *exc):
-        from fasterseg_b200 import _lib
-        for k, v in self.saved.items():
-            _lib.set_option(k, v)
-
-
-# ---- operands -------------------------------------------------------------------------------------------------------------------
-def _ints(shape, gen):
-    """sparse integers in {-1, 0, 1}: P(-1) = P(1) = 1/8"""
-    v = torch.randint(0, 8, shape, generator=gen, device="cuda")
-    return ((v == 1).to(torch.int8) - (v == 0).to(torch.int8)).to(F64)
-
-
-def _normal(shape, gen):
-    return torch.randn(shape, generator=gen, device="cuda", dtype=torch.float32).half().to(F64)
-
-
-class Slice:
-    """channels [off, off + C) of an NHWC buffer of pixel stride cs, with one spare pixel after the end"""
-
-    def __init__(self, N, H, W, C, cs, off, dtype, fill_own, fill_other):
-        self.shape, self.C, self.off = (N, H, W), C, off
-        P = N * H * W
-        self.flat = torch.full(((P + 1) * cs,), fill_other, dtype=dtype, device="cuda")
-        self.buf = self.flat[:P * cs].view(N, H, W, cs)
-        self.view = self.buf[..., off:off + C]
-        if fill_own is not None:
-            self.view.fill_(fill_own)
-
-    def ptr(self):
-        return self.view.data_ptr()
-
-    def put(self, nchw):
-        self.view.copy_(nchw.permute(0, 2, 3, 1).to(self.flat.dtype))
-        return self
-
-    def nchw(self):
-        return self.view.permute(0, 3, 1, 2).to(F64)
-
-    def bits(self):
-        return self.flat.view(torch.int16 if self.flat.element_size() == 2 else torch.int32)
-
-
-def _bits32(t):
-    return t.view(torch.int32)
 
 
 def _ref_dgrad(g, dy, w):
@@ -386,12 +229,6 @@ def _run_exact(geoms, op, seed0):
     _assert_kernels(k.counts, expected)
 
 
-def _assert_kernels(counts, expected):
-    """exactly the expected launches of the library's kernels, by name"""
-    expected = +collections.Counter(expected)
-    assert dict(counts) == dict(expected), "kernels that ran %s, expected %s" % (dict(counts), dict(expected))
-
-
 # ---- the census ----------------------------------------------------------------------------------------------------------------
 def _census(op):
     return [G.from_census(g) for g in CC.geometries() if g["op"] == op]
@@ -497,11 +334,6 @@ def _random_dgrad(g, seed):
         own[:-(g.dxcs + 8)].view(g.N, g.H, g.W, g.dxcs + 8)[..., 8:8 + g.Cin] = True
         assert torch.equal(xs.bits()[~own], before[~own]), "%r %s: dx sentinels overwritten" % (g, path)
     return worst
-
-
-def _report(name, worst):
-    print("%s worst err/bound: %s" % (name, ", ".join("%s %.3f" % kv for kv in sorted(worst.items()))))
-    assert max(worst.values()) <= 1.0, worst
 
 
 @pytest.mark.parametrize("gscale", [1024.0, 3.0])
