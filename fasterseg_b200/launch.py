@@ -278,6 +278,44 @@ def install_dataloader_patch(script):
     return finder
 
 
+def install_criterion_patch(script):
+    """Training criterion without host syncs (losses.install_reference_ohem): when the driver imports the reference's
+    seg_opr.loss_opr from the tools/ directory next to its own (train.py:27, train_search.py), patch
+    ProbOhemCrossEntropy2d.forward.  Returns the finder, or None (and changes nothing) when no reference tools/ directory is
+    found."""
+    tools = reference_tools_dir(script)
+    if tools is None:
+        return None
+    from . import losses
+    finder = _PatchAfterImport("seg_opr.loss_opr", os.path.join(tools, "seg_opr", "loss_opr.py"), losses.install_reference_ohem)
+    sys.meta_path.insert(0, finder)
+    return finder
+
+
+def install_train_metrics_patch(script):
+    """Per-step training mIoU on the device (fasterseg_b200.train_metrics): when the driver imports the `seg_metrics` module
+    next to it (train/seg_metrics.py), patch Seg_Metrics.update.  Returns the finder, or None (and changes nothing) when the
+    script's directory has no seg_metrics.py."""
+    path = os.path.join(os.path.dirname(os.path.abspath(script)), "seg_metrics.py")
+    if not os.path.isfile(path):
+        return None
+    from . import train_metrics
+    finder = _PatchAfterImport("seg_metrics", path, train_metrics.install)
+    sys.meta_path.insert(0, finder)
+    return finder
+
+
+def install_lazy_logits_default(script):
+    """Every train/ Network_Multi_Path_Infer the driver builds returns losses.LazyLogits (an instance's own `lazy_logits` still
+    wins): the patched criteria and metric take them without materialising label-resolution logits.  Not for the latency/
+    variant, which has no lazy path.  Returns whether the default was switched on."""
+    if "latency_variant" in shadow_module_names(script)["model_seg"]:
+        return False
+    from . import model_seg
+    model_seg.LAZY_LOGITS = True
+    return True
+
+
 def main(argv=None):
     argv = list(sys.argv[1:] if argv is None else argv)
     if not argv:
@@ -290,6 +328,9 @@ def main(argv=None):
     install_data_parallel()
     install_evaluator_patch(script)
     install_dataloader_patch(script)
+    install_criterion_patch(script)
+    install_train_metrics_patch(script)
+    install_lazy_logits_default(script)
     from . import optim
     optim.install()      # torch.optim.SGD / nn.utils.clip_grad_norm_ take the flat path after a captured `_loss` (torch's otherwise)
     sys.argv = argv

@@ -64,6 +64,11 @@ class Cell(nn.Module):
         return self._op.forward_latency(size)
 
 
+# Default of `Network_Multi_Path_Infer.lazy_logits` for instances that do not set their own.  Off for programs that build the
+# network themselves; the launcher switches it on for the train/ drivers, whose criteria and metric take the lazy logits.
+LAZY_LOGITS = False
+
+
 class Network_Multi_Path_Infer(nn.Module):
     _cell_cls = Cell   # the latency/ variant (latency_variant/model_seg.py) builds its cells from its own operators
 
@@ -358,7 +363,7 @@ class Network_Multi_Path_Infer(nn.Module):
         return self._forward(input)
 
     def _forward(self, input):
-        lazy = self.__dict__.get("lazy_logits", False)   # N1: hand the criteria the low-resolution logits (losses.LazyLogits)
+        lazy = self.__dict__.get("lazy_logits", LAZY_LOGITS)   # N1: hand the criteria the low-resolution logits (losses.LazyLogits)
         if lazy:
             from .losses import LazyLogits
         if not self.training:
