@@ -61,11 +61,13 @@ _SIGS = {
     "fsb_pack_conv_weight": (C.c_int, [C.POINTER(ConvDesc), _P, C.c_int64, C.c_int64, _P, _P]),
     "fsb_bn_fold": (C.c_int, [C.c_int, _P, _P, _P, _P, C.c_float, _P, _P, _P, _P]),
     "fsb_conv_fwd": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, _P]),
+    "fsb_conv_fwd_half": (C.c_int, [C.POINTER(ConvDesc), _P, _P, _P, _P, _P, _P, C.c_int, _P]),
     "fsb_stem_conv_nchw": (C.c_int, [C.c_int] * 4 + [_P, C.c_int, _P, _P, _P, _P, C.c_int, C.c_uint32, _P]),
     "fsb_stem_conv_u8hwc": (C.c_int, [C.c_int] * 4 + [_P, _P, _P, _P, _P, _P, C.c_int, C.c_uint32, _P]),
     "fsb_stem_fused": (C.c_int, [C.c_int] * 4 + [_P, _P, C.c_int, _P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
     "fsb_confusion_matrix": (C.c_int, [C.c_int64, _P, _P, C.c_int, C.c_int, _P, _P]),
     "fsb_bilinear_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, C.c_uint32, _P]),
+    "fsb_bilinear_fwd_half": (C.c_int, [C.c_int] * 4 + [_P, C.c_int, _P, C.c_int, _P, C.c_int, C.c_uint32, _P]),
     "fsb_upsample_logits_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_argmax": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),
     "fsb_upsample_argmax_confusion": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P, _P]),

@@ -101,6 +101,7 @@ int stem_fused_launch(int, int, int, int, const void*, const void*, int, const f
                       const float*, const float*, void*, int, cudaStream_t);
 int confusion_launch(int64_t, const uint8_t*, const void*, int, int, long long*, cudaStream_t);
 int bilinear_launch(int, int, int, int, int, int, const void*, int, void*, int, uint32_t, cudaStream_t);
+int bilinear_up2_half_launch(int, int, int, int, const void*, int, void*, int, void*, int, uint32_t, cudaStream_t);
 int upsample_logits_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
 int upsample_argmax_confusion_launch(int, int, int, int, int, int, const void*, int, const void*, int, long long*, cudaStream_t);
@@ -307,6 +308,24 @@ int fsb_conv_fwd(const fsb_conv_desc* d, const void* x, const void* wpacked, con
   return conv_tc_launch(plan, d, x, wpacked, scale, shift, y, stats, st);
 }
 
+int fsb_conv_fwd_half(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift, void* y,
+                      void* y_half, int y_half_cstride, void* stream) {
+  int rc = check_desc(d);
+  if (rc) return rc;
+  if (!x || !wpacked || !y || !y_half) return set_error(FSB_ERR_INVALID, "conv_fwd_half: null pointer");
+  if (y_half_cstride < d->Cout || (y_half_cstride % 8) || (reinterpret_cast<uintptr_t>(y_half) & 15))
+    return set_error(FSB_ERR_INVALID, "conv_fwd_half: y_half_cstride must be >= Cout and a multiple of 8, y_half 16-byte aligned");
+  if (d->flags & (FSB_CONV_STATS | FSB_CONV_OUT_F32 | FSB_CONV_Y_UP2 | FSB_CONV_X_DOWN2 | FSB_CONV_FORCE_DIRECT))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd_half: no FSB_CONV_STATS / OUT_F32 / Y_UP2 / X_DOWN2 / FORCE_DIRECT");
+  if ((d->Ho % 2) || (d->Wo % 2) || d->Ho > kBilinearLocalMax || d->Wo > kBilinearLocalMax)
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd_half: Ho and Wo must be even and at most kBilinearLocalMax");
+  const ConvPlan plan = conv_plan(d);
+  if (plan.rc) return plan.rc;
+  if (plan.direct) return set_error(FSB_ERR_UNSUPPORTED, "conv_fwd_half: this problem runs on the direct kernel");
+  const ConvHalfOut half = {y_half, y_half_cstride};
+  return conv_tc_launch(plan, d, x, wpacked, scale, shift, y, nullptr, static_cast<cudaStream_t>(stream), nullptr, &half);
+}
+
 int fsb_stem_conv_nchw(int N, int H, int W, int Cout, const void* x, int x_is_f32, const float* w, const float* scale,
                        const float* shift, void* y, int y_cstride, uint32_t flags, void* stream) {
   if (N <= 0 || H <= 0 || W <= 0 || Cout <= 0 || !x || !w || !y || y_cstride < Cout)
@@ -338,6 +357,12 @@ int fsb_bilinear_fwd(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x
                      void* stream) {
   if (N <= 0 || C <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !y) return set_error(FSB_ERR_INVALID, "bilinear: bad argument");
   return bilinear_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, y, ycs, flags, static_cast<cudaStream_t>(stream));
+}
+
+int fsb_bilinear_fwd_half(int N, int C, int Hi, int Wi, const void* x, int xcs, void* y, int ycs, void* y_half, int yhcs,
+                          uint32_t flags, void* stream) {
+  if (N <= 0 || C <= 0 || Hi <= 0 || Wi <= 0 || !x || !y || !y_half) return set_error(FSB_ERR_INVALID, "bilinear_fwd_half: bad argument");
+  return bilinear_up2_half_launch(N, C, Hi, Wi, x, xcs, y, ycs, y_half, yhcs, flags, static_cast<cudaStream_t>(stream));
 }
 
 int fsb_upsample_logits_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int out_dtype,

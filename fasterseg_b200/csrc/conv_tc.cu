@@ -74,6 +74,16 @@ struct ConvTcUp2Params {
   CUtensorMap tmap_up[6];
 };
 
+// Parameters of the half-output instances (fsb_conv_fwd_half): besides y, the epilogue stores bilinear(y, (Ho/2, Wo/2),
+// align_corners=True) to y_half.  A struct of its own for the same reason as ConvTcUp2Params.
+struct ConvTcHalfParams {
+  ConvTcParams p;
+  __half* y_half;
+  int y_half_cstride;
+  int Hh, Wh;     // Ho / 2, Wo / 2
+  float sh, sw;   // ac_scale(Ho, Hh), ac_scale(Wo, Wh)
+};
+
 // shared memory after the main loop: [0, kOutBytes) = statistics partials or the TMA-store staging slabs,
 // [kOutBytes, + NT * kAccLd * 4) = the parked accumulator; both reuse the (then idle) stage ring
 __host__ __device__ constexpr uint32_t conv_tc_out_bytes(int nt) { return static_cast<uint32_t>((nt + 63) / 64) * kTileM * 128; }
@@ -89,10 +99,11 @@ __host__ __device__ constexpr uint32_t conv_tc_epilogue_bytes(int nt) { return c
 //   16 x 8 tiles: half h = the 8 x 8 block at columns 8h..8h+7, groups = tile rows (stride tw + 2 pixels);
 //   8 x 16 tiles: half h = tile rows 8h..8h+7, groups = tile rows (stride tw + 2 pixels).
 
-// The kernel body.  UP2 (FSB_CONV_Y_UP2) only adds the stores of each staged slab to lattices 1 .. y_reps - 1; it is compiled
-// into instances of its own (conv_tc_up2_kernel) so that the instances every other call runs keep their registers.
-template <int BK, int NT, bool WIN, bool UP2>
-__device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtensorMap* tmap_up, int y_reps) {
+// The kernel body.  UP2 (FSB_CONV_Y_UP2) only adds the stores of each staged slab to lattices 1 .. y_reps - 1, HALF the /2 output
+// read back from each staged slab; both are compiled into instances of their own (conv_tc_up2_kernel, conv_tc_half_kernel) so
+// that the instances every other call runs keep their registers.
+template <int BK, int NT, bool WIN, bool UP2, bool HALF>
+__device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtensorMap* tmap_up, int y_reps, const ConvTcHalfParams* hp) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t full_bar[kMaxStages];
   __shared__ __align__(8) uint64_t empty_bar[kMaxStages];
@@ -393,6 +404,31 @@ __device__ __forceinline__ void conv_tc_body(const ConvTcParams& p, const CUtens
                            h0, img);
           tma_store_commit();
         }
+        if constexpr (HALF) {
+          // bilinear /2 of the staged slab: the tile starts on even rows and columns and a /2 pixel reads only its own 2x2
+          // block (kBilinearLocalMax), so the tile's (th / 2) x (tw / 2) pixels need no halo.  One item = one /2 pixel x 8
+          // channels; the slab is only read here, while the TMA engine reads it too.
+          const int vecs = ((NT - c0) >= 64 ? 64 : p.tail_w) >> 3;
+          const uint8_t* slab = smem + static_cast<size_t>(c0 >> 6) * (kTileM * 128);
+          const int hw = p.tw >> 1;
+          for (int it = threadIdx.x; it < (kTileM / 4) * vecs; it += kMmaThreads) {
+            const int v = it % vecs, hpix = it / vecs;
+            const int oi = (h0 >> 1) + hpix / hw, oj = (w0 >> 1) + hpix % hw;
+            const int ch = n0 + c0 + v * 8;
+            if (oi >= hp->Hh || oj >= hp->Wh || ch >= p.Cout) continue;
+            int r0, r1, q0, q1;
+            float lh, lw;
+            src_index(oi, hp->sh, p.Ho, r0, r1, lh);
+            src_index(oj, hp->sw, p.Wo, q0, q1, lw);
+            auto px = [&](int r, int q) {
+              const int mm = (r - h0) * p.tw + (q - w0);
+              return *reinterpret_cast<const uint4*>((NT - c0) >= 64 ? slab + mm * 128 + ((v ^ (mm & 7)) << 4)
+                                                                      : slab + mm * (p.tail_w * 2) + (v << 4));
+            };
+            *reinterpret_cast<uint4*>(hp->y_half + (static_cast<size_t>(img) * hp->Hh * hp->Wh + static_cast<size_t>(oi) * hp->Wh + oj) *
+                                                       hp->y_half_cstride + ch) = bilinear8(px(r0, q0), px(r0, q1), px(r1, q0), px(r1, q1), lh, lw, false);
+          }
+        }
       }
     }  // 64-column batch
     if (p.tma_store && threadIdx.x == 0) tma_store_wait_read();  // smem must outlive the bulk reads
@@ -423,13 +459,19 @@ __host__ __device__ constexpr int conv_tc_residency(int nt) { return nt <= 64 ? 
 template <int BK, int NT, bool WIN>
 __global__ void __launch_bounds__(kThreads, conv_tc_residency(NT))
 conv_tc_kernel(const __grid_constant__ ConvTcParams p) {
-  conv_tc_body<BK, NT, WIN, false>(p, nullptr, 1);
+  conv_tc_body<BK, NT, WIN, false, false>(p, nullptr, 1, nullptr);
 }
 
 template <int BK, int NT, bool WIN>
 __global__ void __launch_bounds__(kThreads, conv_tc_residency(NT))
 conv_tc_up2_kernel(const __grid_constant__ ConvTcUp2Params q) {
-  conv_tc_body<BK, NT, WIN, true>(q.p, q.tmap_up, q.y_reps);
+  conv_tc_body<BK, NT, WIN, true, false>(q.p, q.tmap_up, q.y_reps, nullptr);
+}
+
+template <int BK, int NT, bool WIN>
+__global__ void __launch_bounds__(kThreads, conv_tc_residency(NT))
+conv_tc_half_kernel(const __grid_constant__ ConvTcHalfParams q) {
+  conv_tc_body<BK, NT, WIN, false, true>(q.p, nullptr, 1, &q);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -607,31 +649,34 @@ ConvPlan conv_plan(const fsb_conv_desc* d, const ConvTcCustom* cu, bool window_o
   return pl;
 }
 
-// The kernel instance a plan runs: (BK, NT, WIN) and, for FSB_CONV_Y_UP2, conv_tc_up2_kernel.  The launch and the occupancy
-// query both select it here; entry is the pointer of the two that the plan runs, its dynamic shared-memory limit raised.
+// The kernel instance a plan runs: (BK, NT, WIN) and, for FSB_CONV_Y_UP2, conv_tc_up2_kernel, for a half-resolution output
+// conv_tc_half_kernel.  The launch and the occupancy query both select it here; entry is the pointer of the three that the
+// launch runs, its dynamic shared-memory limit raised.
 struct ConvTcInstance {
   void (*plain)(ConvTcParams);
   void (*up2)(ConvTcUp2Params);
+  void (*half)(ConvTcHalfParams);
   const void* entry;
 };
 
 template <int BK, bool WIN>
 static ConvTcInstance conv_tc_instance_nt(int n_tile) {
   switch (n_tile) {
-    case 16: return {conv_tc_kernel<BK, 16, WIN>, conv_tc_up2_kernel<BK, 16, WIN>, nullptr};
-    case 32: return {conv_tc_kernel<BK, 32, WIN>, conv_tc_up2_kernel<BK, 32, WIN>, nullptr};
-    case 48: return {conv_tc_kernel<BK, 48, WIN>, conv_tc_up2_kernel<BK, 48, WIN>, nullptr};
-    case 64: return {conv_tc_kernel<BK, 64, WIN>, conv_tc_up2_kernel<BK, 64, WIN>, nullptr};
-    case 96: return {conv_tc_kernel<BK, 96, WIN>, conv_tc_up2_kernel<BK, 96, WIN>, nullptr};
-    default: return {conv_tc_kernel<BK, 128, WIN>, conv_tc_up2_kernel<BK, 128, WIN>, nullptr};
+    case 16: return {conv_tc_kernel<BK, 16, WIN>, conv_tc_up2_kernel<BK, 16, WIN>, conv_tc_half_kernel<BK, 16, WIN>, nullptr};
+    case 32: return {conv_tc_kernel<BK, 32, WIN>, conv_tc_up2_kernel<BK, 32, WIN>, conv_tc_half_kernel<BK, 32, WIN>, nullptr};
+    case 48: return {conv_tc_kernel<BK, 48, WIN>, conv_tc_up2_kernel<BK, 48, WIN>, conv_tc_half_kernel<BK, 48, WIN>, nullptr};
+    case 64: return {conv_tc_kernel<BK, 64, WIN>, conv_tc_up2_kernel<BK, 64, WIN>, conv_tc_half_kernel<BK, 64, WIN>, nullptr};
+    case 96: return {conv_tc_kernel<BK, 96, WIN>, conv_tc_up2_kernel<BK, 96, WIN>, conv_tc_half_kernel<BK, 96, WIN>, nullptr};
+    default: return {conv_tc_kernel<BK, 128, WIN>, conv_tc_up2_kernel<BK, 128, WIN>, conv_tc_half_kernel<BK, 128, WIN>, nullptr};
   }
 }
 
-static int conv_tc_instance(const ConvPlan& pl, ConvTcInstance* k) {
+static int conv_tc_instance(const ConvPlan& pl, ConvTcInstance* k, bool half = false) {
   if (pl.win) *k = conv_tc_instance_nt<64, true>(pl.n_tile);
   else if (pl.bk == 64) *k = conv_tc_instance_nt<64, false>(pl.n_tile);
   else *k = conv_tc_instance_nt<32, false>(pl.n_tile);
-  k->entry = pl.up2 ? reinterpret_cast<const void*>(k->up2) : reinterpret_cast<const void*>(k->plain);
+  k->entry = pl.up2 ? reinterpret_cast<const void*>(k->up2)
+                    : (half ? reinterpret_cast<const void*>(k->half) : reinterpret_cast<const void*>(k->plain));
   return ensure_dyn_smem(k->entry, 220 * 1024, "cudaFuncSetAttribute(conv_tc)");
 }
 
@@ -644,8 +689,11 @@ int conv_tc_occupancy(const ConvPlan& plan) {
 }
 
 int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale,
-                   const float* shift, void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu) {
+                   const float* shift, void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu, const ConvHalfOut* half) {
   if (plan.rc) return plan.rc;
+  if (half && (cu || plan.up2 || (d->flags & FSB_CONV_X_DOWN2)))
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: a half-resolution output cannot be combined with a custom lattice, FSB_CONV_Y_UP2 or "
+                                          "FSB_CONV_X_DOWN2");
   if ((reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(wpacked) & 15))
     return set_error(FSB_ERR_INVALID, "conv_tc: x / wpacked must be 16-byte aligned");
   const ConvGeom g = conv_geom(d);
@@ -718,6 +766,9 @@ int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, 
     p.tma_store = 1;
   }
   if (cu && !p.tma_store) return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: custom output lattice needs the TMA-store epilogue");
+  if (half && !p.tma_store)
+    return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: a half-resolution output needs the TMA-store epilogue (fp16 output, Cout and "
+                                          "y_cstride multiples of 8, 16-byte aligned y)");
   if (plan.up2 && !p.tma_store)
     return set_error(FSB_ERR_UNSUPPORTED, "conv_tc: FSB_CONV_Y_UP2 needs the TMA-store epilogue (fp16 output, Cout and y_cstride "
                                           "multiples of 8, 16-byte aligned y)");
@@ -786,10 +837,24 @@ int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, 
     if (rc) return rc;
   }
   ConvTcInstance k;
-  if (int rc = conv_tc_instance(plan, &k)) return rc;
+  if (int rc = conv_tc_instance(plan, &k, half != nullptr)) return rc;
   const dim3 grid(static_cast<unsigned>(plan.m_tiles), static_cast<unsigned>(plan.n_tiles));
-  const cudaError_t e = plan.up2 ? launch_kernel(k.up2, grid, dim3(kThreads), plan.smem, stream, q)
-                                 : launch_kernel(k.plain, grid, dim3(kThreads), plan.smem, stream, q.p);
+  cudaError_t e;
+  if (half) {
+    ConvTcHalfParams hq;
+    memset(&hq, 0, sizeof(hq));
+    hq.p = p;
+    hq.y_half = static_cast<__half*>(half->y);
+    hq.y_half_cstride = half->cstride;
+    hq.Hh = plan.Ho / 2;
+    hq.Wh = plan.Wo / 2;
+    hq.sh = ac_scale(plan.Ho, hq.Hh);
+    hq.sw = ac_scale(plan.Wo, hq.Wh);
+    e = launch_kernel(k.half, grid, dim3(kThreads), plan.smem, stream, hq);
+  } else {
+    e = plan.up2 ? launch_kernel(k.up2, grid, dim3(kThreads), plan.smem, stream, q)
+                 : launch_kernel(k.plain, grid, dim3(kThreads), plan.smem, stream, q.p);
+  }
   return e == cudaSuccess ? FSB_OK : set_cuda_error(e, "conv_tc launch");
 }
 

@@ -248,4 +248,45 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
+// ------------------------------------------------------------------------------------------
+// bilinear (align_corners=True) interpolation, shared by every kernel that stores a bilinear_nhwc_kernel value (resize.cu,
+// and the half-resolution output of conv_tc), so that a fused value is the same code on the same fp16 inputs.
+// Coordinate rule (ATen area_pixel_compute_source_index, align_corners): src = dst * (in - 1) / (out - 1) [scale in fp32,
+// 0 if out == 1]; i0 = floor(src); l1 = src - i0.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ void src_index(int dst, float scale, int n_in, int& i0, int& i1, float& l1) {
+  const float src = scale * static_cast<float>(dst);
+  i0 = static_cast<int>(src);
+  if (i0 > n_in - 1) i0 = n_in - 1;
+  i1 = i0 + (i0 < n_in - 1 ? 1 : 0);
+  l1 = src - static_cast<float>(i0);
+}
+__host__ __device__ inline float ac_scale(int n_in, int n_out) {
+  return n_out > 1 ? static_cast<float>(n_in - 1) / static_cast<float>(n_out - 1) : 0.f;
+}
+// 8 channels of one output pixel from the four source pixels (rows h0 / h1, columns w0 / w1) and the weights lh, lw of
+// src_index: fp32 arithmetic, optional ReLU, fp16 result
+__device__ __forceinline__ uint4 bilinear8(const uint4& v00, const uint4& v01, const uint4& v10, const uint4& v11, float lh, float lw,
+                                           bool relu) {
+  const __half2* a = reinterpret_cast<const __half2*>(&v00);
+  const __half2* b = reinterpret_cast<const __half2*>(&v01);
+  const __half2* c = reinterpret_cast<const __half2*>(&v10);
+  const __half2* d = reinterpret_cast<const __half2*>(&v11);
+  const float w00 = (1.f - lh) * (1.f - lw), w01 = (1.f - lh) * lw, w10 = lh * (1.f - lw), w11 = lh * lw;
+  uint4 out;
+  uint32_t* o = reinterpret_cast<uint32_t*>(&out);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 fa = __half22float2(a[j]), fb = __half22float2(b[j]), fc = __half22float2(c[j]), fd = __half22float2(d[j]);
+    float r0 = w00 * fa.x + w01 * fb.x + w10 * fc.x + w11 * fd.x;
+    float r1 = w00 * fa.y + w01 * fb.y + w10 * fc.y + w11 * fd.y;
+    if (relu) {
+      r0 = fmaxf(r0, 0.f);
+      r1 = fmaxf(r1, 0.f);
+    }
+    o[j] = pack_half2(r0, r1);
+  }
+  return out;
+}
+
 }  // namespace fsb

@@ -114,9 +114,21 @@ struct ConvPlan {
 // window_ok = false keeps a 3x3 stride-1 problem on the per-tap mode unless FSB_CONV_TC2 forces the window mode; cu (custom tap
 // tables) always runs per-tap
 ConvPlan conv_plan(const fsb_conv_desc* d, const ConvTcCustom* cu = nullptr, bool window_ok = true);
-// launch conv_tc as planned (plan = conv_plan(d, cu, ...), not direct)
+// Largest output extent (rows or columns) at which a bilinear /2 of it is local to 2x2 blocks and an exact x2 upsample of
+// half of it reads at most 3 x 3 source pixels per 2x2 output block: checked for every even extent up to here with the fp32
+// index rule of src_index (fsb_common.cuh, tests/test_resize_fusion_cpu.py).  At 4164 the fp32 rounding of src already moves a
+// /2 footprint out of its block.
+constexpr int kBilinearLocalMax = 4096;
+
+// second output of fsb_conv_fwd_half: bilinear(y, (Ho / 2, Wo / 2), align_corners=True), NHWC fp16 with pixel stride cstride
+struct ConvHalfOut {
+  void* y;
+  int cstride;
+};
+// launch conv_tc as planned (plan = conv_plan(d, cu, ...), not direct); half: also store the /2 output (even Ho, Wo)
 int conv_tc_launch(const ConvPlan& plan, const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale,
-                   const float* shift, void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr);
+                   const float* shift, void* y, float* stats, cudaStream_t stream, const ConvTcCustom* cu = nullptr,
+                   const ConvHalfOut* half = nullptr);
 // CTAs per SM of the planned conv_tc launch, from the CUDA occupancy calculator; launches nothing
 int conv_tc_occupancy(const ConvPlan& plan);
 int conv_wgrad_tc_supported(const fsb_conv_desc* d, int dy_cstride);

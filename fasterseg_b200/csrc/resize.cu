@@ -1,23 +1,11 @@
 // resize.cu -- K4 / K9: bilinear (align_corners=True) resize kernels and layout plumbing, all HBM-bound:
 // 16-byte vector loads/stores over the channel dimension of NHWC fp16, fp32 interpolation arithmetic.
 // Reference call sites: F.interpolate at search/operations.py:271,275,437,444; search/model_search.py:339-343,353-357;
-// train/model_seg.py:305,310,317,359-365.  Coordinate rule (ATen area_pixel_compute_source_index, align_corners):
-//   src = dst * (in - 1) / (out - 1)  [scale computed in fp32, 0 if out == 1];  i0 = floor(src); l1 = src - i0.
+// train/model_seg.py:305,310,317,359-365.  Coordinate rule and interpolation: src_index / bilinear8 (fsb_common.cuh).
 #include "fsb_common.cuh"
 #include "fsb_internal.h"
 
 namespace fsb {
-
-__device__ __forceinline__ void src_index(int dst, float scale, int n_in, int& i0, int& i1, float& l1) {
-  const float src = scale * static_cast<float>(dst);
-  i0 = static_cast<int>(src);
-  if (i0 > n_in - 1) i0 = n_in - 1;
-  i1 = i0 + (i0 < n_in - 1 ? 1 : 0);
-  l1 = src - static_cast<float>(i0);
-}
-__host__ __device__ inline float ac_scale(int n_in, int n_out) {
-  return n_out > 1 ? static_cast<float>(n_in - 1) / static_cast<float>(n_out - 1) : 0.f;
-}
 
 // one thread = one output pixel x 8 channels
 __global__ void __launch_bounds__(256)
@@ -43,25 +31,75 @@ bilinear_nhwc_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half*
   const uint4 v01 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h0) * Wi + w1) * xcs);
   const uint4 v10 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h1) * Wi + w0) * xcs);
   const uint4 v11 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h1) * Wi + w1) * xcs);
-  const __half2* a = reinterpret_cast<const __half2*>(&v00);
-  const __half2* b = reinterpret_cast<const __half2*>(&v01);
-  const __half2* c = reinterpret_cast<const __half2*>(&v10);
-  const __half2* d = reinterpret_cast<const __half2*>(&v11);
-  const float w00 = (1.f - lh) * (1.f - lw), w01 = (1.f - lh) * lw, w10 = lh * (1.f - lw), w11 = lh * lw;
-  uint4 out;
-  uint32_t* o = reinterpret_cast<uint32_t*>(&out);
+  *reinterpret_cast<uint4*>(y + static_cast<size_t>(pix) * ycs + cv * 8) = bilinear8(v00, v01, v10, v11, lh, lw, relu != 0);
+}
+
+// Exact x2 upsample (Ho = 2Hi, Wo = 2Wi) that also stores the bilinear /2 of its own output (Hi x Wi, y_half): one thread = one
+// 2x2 output block x 8 channels.  Each of the four outputs is bilinear_nhwc_kernel's value; the /2 pixel (k, l) reads only rows
+// 2k, 2k+1 and columns 2l, 2l+1 of the output (kBilinearLocalMax), i.e. this thread's four fp16 results.
+__global__ void __launch_bounds__(256)
+bilinear_up2_half_nhwc_kernel(int N, int C, int Hi, int Wi, const __half* __restrict__ x, int xcs, __half* __restrict__ y, int ycs,
+                              __half* __restrict__ yh, int yhcs, float sh, float sw, float dh, float dw, int relu) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int cvec = C >> 3;
+  const int64_t total = static_cast<int64_t>(N) * Hi * Wi * cvec;
+  const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (gid >= total) return;
+  const int cv = static_cast<int>(gid % cvec);
+  const int64_t blk = gid / cvec;
+  const int l = static_cast<int>(blk % Wi);
+  const int k = static_cast<int>((blk / Wi) % Hi);
+  const int n = static_cast<int>(blk / (static_cast<int64_t>(Wi) * Hi));
+  const int Ho = 2 * Hi, Wo = 2 * Wi;
+  const __half* base = x + static_cast<size_t>(n) * Hi * Wi * xcs + cv * 8;
+  __half* ybase = y + static_cast<size_t>(n) * Ho * Wo * ycs + cv * 8;
+  uint4 r[2][2];
 #pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 fa = __half22float2(a[j]), fb = __half22float2(b[j]), fc = __half22float2(c[j]), fd = __half22float2(d[j]);
-    float r0 = w00 * fa.x + w01 * fb.x + w10 * fc.x + w11 * fd.x;
-    float r1 = w00 * fa.y + w01 * fb.y + w10 * fc.y + w11 * fd.y;
-    if (relu) {
-      r0 = fmaxf(r0, 0.f);
-      r1 = fmaxf(r1, 0.f);
+  for (int a = 0; a < 2; ++a) {
+    int h0, h1;
+    float lh;
+    src_index(2 * k + a, sh, Hi, h0, h1, lh);
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+      int w0, w1;
+      float lw;
+      src_index(2 * l + b, sw, Wi, w0, w1, lw);
+      const uint4 v00 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h0) * Wi + w0) * xcs);
+      const uint4 v01 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h0) * Wi + w1) * xcs);
+      const uint4 v10 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h1) * Wi + w0) * xcs);
+      const uint4 v11 = *reinterpret_cast<const uint4*>(base + (static_cast<size_t>(h1) * Wi + w1) * xcs);
+      r[a][b] = bilinear8(v00, v01, v10, v11, lh, lw, relu != 0);
+      *reinterpret_cast<uint4*>(ybase + (static_cast<size_t>(2 * k + a) * Wo + 2 * l + b) * ycs) = r[a][b];
     }
-    o[j] = pack_half2(r0, r1);
   }
-  *reinterpret_cast<uint4*>(y + static_cast<size_t>(pix) * ycs + cv * 8) = out;
+  int h0, h1, w0, w1;
+  float lh, lw;
+  src_index(k, dh, Ho, h0, h1, lh);
+  src_index(l, dw, Wo, w0, w1, lw);
+  auto at = [&](int hh, int ww) {  // selects, not a dynamically indexed (local-memory) array
+    const bool a = hh != 2 * k, b = ww != 2 * l;
+    return a ? (b ? r[1][1] : r[1][0]) : (b ? r[0][1] : r[0][0]);
+  };
+  *reinterpret_cast<uint4*>(yh + (static_cast<size_t>(n) * Hi * Wi + static_cast<size_t>(k) * Wi + l) * yhcs + cv * 8) =
+      bilinear8(at(h0, w0), at(h0, w1), at(h1, w0), at(h1, w1), lh, lw, false);
+}
+
+int bilinear_up2_half_launch(int N, int C, int Hi, int Wi, const void* x, int xcs, void* y, int ycs, void* y_half, int yhcs,
+                             uint32_t flags, cudaStream_t stream) {
+  if (C % 8 || xcs % 8 || ycs % 8 || yhcs % 8 || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15) ||
+      (reinterpret_cast<uintptr_t>(y_half) & 15))
+    return set_error(FSB_ERR_INVALID, "bilinear_fwd_half: C, strides must be multiples of 8 and pointers 16B aligned");
+  if (2 * Hi > kBilinearLocalMax || 2 * Wi > kBilinearLocalMax)
+    return set_error(FSB_ERR_UNSUPPORTED, "bilinear_fwd_half: output extent beyond kBilinearLocalMax");
+  const int64_t total = static_cast<int64_t>(N) * Hi * Wi * (C / 8);
+  const int64_t blocks = (total + 255) / 256;
+  FSB_LAUNCH(bilinear_up2_half_nhwc_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, stream,
+      N, C, Hi, Wi, static_cast<const __half*>(x), xcs, static_cast<__half*>(y), ycs, static_cast<__half*>(y_half), yhcs,
+      ac_scale(Hi, 2 * Hi), ac_scale(Wi, 2 * Wi), ac_scale(2 * Hi, Hi), ac_scale(2 * Wi, Wi), (flags & FSB_CONV_RELU) ? 1 : 0);
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "bilinear_fwd_half launch");
+  return FSB_OK;
 }
 
 int bilinear_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, void* y, int ycs, uint32_t flags,

@@ -127,8 +127,10 @@ def active_bn(bn):
 
 
 def conv_bn_act(x: torch.Tensor, conv: nn.Conv2d, bn: Optional[nn.BatchNorm2d], relu: bool,
-                out: Optional[torch.Tensor] = None, off=(0, 0)) -> torch.Tensor:
-    """act(BN(conv(x))) on NHWC fp16 views.  `off` = input origin shift (FactorizedReduce, operations.py:523)."""
+                out: Optional[torch.Tensor] = None, off=(0, 0), out_half: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """act(BN(conv(x))) on NHWC fp16 views.  `off` = input origin shift (FactorizedReduce, operations.py:523).  out_half: also
+    write bilinear(y, (Ho // 2, Wo // 2)) there -- from the conv's own epilogue with eval-mode BN (F_.conv_fwd), else by a
+    separate resize."""
     x = F_.to_nhwc_half(x)
     ci, co = active_channels(conv)
     assert x.shape[1] == ci, "input has %d channels, conv expects %d" % (x.shape[1], ci)
@@ -136,12 +138,16 @@ def conv_bn_act(x: torch.Tensor, conv: nn.Conv2d, bn: Optional[nn.BatchNorm2d], 
     assert conv.dilation[0] == 1 and conv.groups == 1, "only dense dilation-1 convs are on the hot path (SURVEY section 0)"
     wp = packed_weight(conv, ci, co)
     bn = active_bn(bn) if bn is not None else None
+    from . import autograd as AG
+    if out_half is not None and ((bn is not None and (bn.training or bn.running_mean is None)) or AG.grad_mode(x, conv.weight)):
+        y = conv_bn_act(x, conv, bn, relu, out=out, off=off)   # batch statistics (SelBN included) or autograd: a separate /2
+        F_.bilinear(y, (y.shape[2] // 2, y.shape[3] // 2), out=out_half)
+        return y
     if isinstance(bn, SelBN):
         from .autograd import conv_bn_act_train_sel
         assert out is None and off == (0, 0)
         return conv_bn_act_train_sel(x, conv, bn, relu, ci, co)
     training = bn is not None and (bn.training or bn.running_mean is None)
-    from . import autograd as AG
     want_grad = AG.grad_mode(x, conv.weight)
     if not training:
         if want_grad and bn is None:
@@ -150,7 +156,8 @@ def conv_bn_act(x: torch.Tensor, conv: nn.Conv2d, bn: Optional[nn.BatchNorm2d], 
             return conv_bias_act(x, conv, relu, ci, co)
         # eval-mode BN: inference only (the teacher runs under no_grad, train/train.py:249-252)
         scale, shift = folded_bn(bn, co, conv.bias)
-        return F_.conv_fwd(x, wp, co, k, s, p, scale, shift, relu=relu, out=out, off=off)
+        half = {} if out_half is None else {"out_half": out_half}   # only where given: wrappers' stand-ins need not know it
+        return F_.conv_fwd(x, wp, co, k, s, p, scale, shift, relu=relu, out=out, off=off, **half)
     if want_grad:
         from .autograd import conv_bn_act_train  # training path with backward
         return conv_bn_act_train(x, conv, bn, relu, ci, co, out=out, off=off)

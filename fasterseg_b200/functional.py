@@ -156,12 +156,14 @@ def rowsum(rows):
 
 
 def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=False, out=None, off=(0, 0),
-             stats=None, force_direct=False, out_f32=False, stats_off=0, down2=False, up2=False):
+             stats=None, force_direct=False, out_f32=False, stats_off=0, down2=False, up2=False, out_half=None):
     """y = act(conv(x) * scale + shift); x/out NHWC fp16 views (see module docstring).  out_f32: fp32 NHWC output (the
     training path's raw conv result, normalised by BatchNorm from un-rounded values).  stats: a `conv_stats_buffer`; this
     conv's per-channel sums land at column stats_off + c, its sums of squares at SC + stats_off + c of every row.
     down2: the conv runs on nearest(x, (H/2, W/2)), read in place from x (even H, W; stride 1).  up2: the result is
-    nearest(y, (2Ho, 2Wo)), written in place (out is the 2Ho x 2Wo map).  Both are bit for bit the separate resize."""
+    nearest(y, (2Ho, 2Wo)), written in place (out is the 2Ho x 2Wo map).  Both are bit for bit the separate resize.
+    out_half: an NHWC fp16 (N, Cout, Ho // 2, Wo // 2) view that also receives bilinear(y, (Ho // 2, Wo // 2)) -- from the conv's
+    own epilogue where the library can (fsb_conv_fwd_half), else from a second launch; the same bits either way."""
     N, Cin, H, W, xcs = nhwc_info(x)
     if down2:
         if H % 2 or W % 2:
@@ -183,6 +185,14 @@ def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=
     if out_f32:
         flags |= FSB_CONV_OUT_F32
     d = ConvDesc(N, H, W, Cin, Cout, ksize, stride, pad, 1, off[0], off[1], Ho, Wo, xcs, ycs, flags)
+    if out_half is not None:
+        _, Ch, Hh, Wh, hcs = nhwc_info(out_half)
+        assert (Ch, Hh, Wh) == (Cout, Ho // 2, Wo // 2) and not up2, ((Ch, Hh, Wh), (Cout, Ho // 2, Wo // 2))
+        rc = _lib.lib().fsb_conv_fwd_half(C.byref(d), _ptr(x), _ptr(wpacked), _ptr(scale), _ptr(shift), _ptr(out), _ptr(out_half),
+                                          hcs, _stream())
+        if rc != _lib.FSB_ERR_UNSUPPORTED:
+            check(rc, "fsb_conv_fwd_half")
+            return out
     if stats is not None:
         assert stats.dim() == 2 and stats.dtype == torch.float32 and stats.is_contiguous()
         d.stats_C, d.stats_off = stats.shape[1] // 2, int(stats_off)
@@ -190,6 +200,8 @@ def conv_fwd(x, wpacked, Cout, ksize, stride, pad, scale=None, shift=None, relu=
         assert rows == stats.shape[0], "statistics buffer has %d rows, this launch writes %d" % (stats.shape[0], rows)
     check(_lib.lib().fsb_conv_fwd(C.byref(d), _ptr(x), _ptr(wpacked), _ptr(scale), _ptr(shift), _ptr(out), _ptr(stats),
                                   _stream()), "fsb_conv_fwd")
+    if out_half is not None:
+        bilinear(out, (Ho // 2, Wo // 2), out=out_half)
     return out
 
 
@@ -373,15 +385,28 @@ def supernet_latency_bwd(plan_host, plan, gout, workspace, grads):
     return grads
 
 
-def bilinear(x, size, relu=False, out=None):
+def bilinear(x, size, relu=False, out=None, out_half=None):
+    """F.interpolate(x, size, mode='bilinear', align_corners=True) (then ReLU if relu).  out_half: an NHWC fp16
+    (N, C, Ho // 2, Wo // 2) view that also receives bilinear(y, (Ho // 2, Wo // 2)) -- for an exact x2 upsample from the same
+    launch (fsb_bilinear_fwd_half), else from a second one; the same bits either way."""
     N, Cc, Hi, Wi, xcs = nhwc_info(x)
     Ho, Wo = int(size[0]), int(size[1])
     if out is None:
         out = empty_nhwc(N, Cc, Ho, Wo, x.device)
     _, Co, Hy, Wy, ycs = nhwc_info(out)
     assert (Co, Hy, Wy) == (Cc, Ho, Wo)
-    check(_lib.lib().fsb_bilinear_fwd(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(out), ycs, FSB_CONV_RELU if relu else 0,
-                                      _stream()), "fsb_bilinear_fwd")
+    flags = FSB_CONV_RELU if relu else 0
+    if out_half is not None:
+        _, Ch, Hh, Wh, hcs = nhwc_info(out_half)
+        assert (Ch, Hh, Wh) == (Cc, Ho // 2, Wo // 2), ((Ch, Hh, Wh), (Cc, Ho // 2, Wo // 2))
+        if (Ho, Wo) == (2 * Hi, 2 * Wi):
+            rc = _lib.lib().fsb_bilinear_fwd_half(N, Cc, Hi, Wi, _ptr(x), xcs, _ptr(out), ycs, _ptr(out_half), hcs, flags, _stream())
+            if rc != _lib.FSB_ERR_UNSUPPORTED:
+                check(rc, "fsb_bilinear_fwd_half")
+                return out
+    check(_lib.lib().fsb_bilinear_fwd(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(out), ycs, flags, _stream()), "fsb_bilinear_fwd")
+    if out_half is not None:
+        bilinear(out, (Ho // 2, Wo // 2), out=out_half)
     return out
 
 

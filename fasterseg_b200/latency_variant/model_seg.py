@@ -40,6 +40,7 @@ class Cell(_train.Cell):
 
 class Network_Multi_Path_Infer(_train.Network_Multi_Path_Infer):
     _cell_cls = Cell
+    fuse_resizes = False   # nearest resizes, folded into the convs' tensor maps instead
 
     def _inference_only(self, input):
         inference_only("Network_Multi_Path_Infer", self.training, input, next(self.parameters(), None))

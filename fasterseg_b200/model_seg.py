@@ -26,7 +26,7 @@ from .decode import (alphas2ops_path_width, betas2path, downs2path, network_meta
                      softmax)
 from .genotypes import PRIMITIVES
 from .operations import *  # noqa: F401,F403  (the reference does `from operations import *`)
-from .operations import OPS, BasicResidual2x, ConvNorm
+from .operations import OPS, BasicResidual2x, ConvNorm, _Residual
 from .seg_oprs import FeatureFusion, Head
 
 BatchNorm2d = nn.BatchNorm2d
@@ -34,6 +34,11 @@ BatchNorm2d = nn.BatchNorm2d
 SCALES = (8, 16, 32)                      # feature strides the decoder tails tap
 _CellStep = namedtuple("_CellStep", "key layer lead members fork")   # one distinct cell of the trunk
 _Tail = namedtuple("_Tail", "branch last")                          # how branch b reaches the 1/8 fusion input
+# Inference outputs a step's producer writes for later kernels (see Network_Multi_Path_Infer._trunk): `half` = steps whose output a
+# zoomed op reads, made by a kernel that also stores the output's bilinear /2; `reads_half` = the zoomed steps that take that /2;
+# `skip` = step -> (branch, link) of the one refine whose concat buffer receives the step's output as its skip feature;
+# `shapes` = each step's output shape.
+_ResizePlan = namedtuple("_ResizePlan", "half reads_half skip shapes")
 
 
 class MixedOp(nn.Module):
@@ -43,8 +48,12 @@ class MixedOp(nn.Module):
         super(MixedOp, self).__init__()
         self._op = OPS[PRIMITIVES[op_idx]](C_in, C_out, stride, slimmable=False, width_mult_list=[1.])
 
-    def forward(self, x, out=None):
-        return self._op(x, out=out) if out is not None else self._op(x)
+    def forward(self, x, out=None, **fused):
+        """fused: out_half / x_half of the residual primitives (operations._Residual.forward), passed on when given"""
+        fused = {k: v for k, v in fused.items() if v is not None}
+        if out is not None:
+            fused["out"] = out
+        return self._op(x, **fused)
 
     def forward_latency(self, size):
         latency, size_out = self._op.forward_latency(size)
@@ -57,8 +66,8 @@ class Cell(nn.Module):
         self._C_in, self._C_out, self._down = C_in, C_out, down
         self._op = MixedOp(C_in, C_out, op_idx, stride=2 if down else 1)
 
-    def forward(self, input, out=None):
-        return self._op(input, out=out)
+    def forward(self, input, out=None, **fused):
+        return self._op(input, out=out, **fused)
 
     def forward_latency(self, size):
         return self._op.forward_latency(size)
@@ -71,6 +80,10 @@ LAZY_LOGITS = False
 
 class Network_Multi_Path_Infer(nn.Module):
     _cell_cls = Cell   # the latency/ variant (latency_variant/model_seg.py) builds its cells from its own operators
+    # Inference on the GPU writes a zoomed op's bilinear /2 input and a refine's skip feature from the kernels that produce them
+    # (_trunk), from the second forward at an input size on.  None: whenever the forward runs in eval mode without autograd on a
+    # CUDA input; False: never; True: also on the stand-in backend of the host tests.  The results are the same bits either way.
+    fuse_resizes = None
 
     def __init__(self, alphas, betas, ratios, num_classes=19, layers=9, criterion=nn.CrossEntropyLoss(ignore_index=-1),
                  Fch=12, width_mult_list=[1., ], stem_head_width=(1., 1.), ignore_skip=False):
@@ -207,6 +220,7 @@ class Network_Multi_Path_Infer(nn.Module):
         # plain (non-Module, non-persistent) attributes: the schedule is derived data
         self.__dict__["_steps"] = steps
         self.__dict__["_tails"] = [_Tail(b, last) for b, last in enumerate(self.lasts)]
+        self.__dict__.pop("_fsb_resize_plans", None)   # recorded per input size from the schedule's first forward (_trunk)
 
     def _tail_modules(self, last):
         """[(arm 1x1, refine 3x3, stride of the coarse input, stride of the skip input, extra skip channels)] for a branch
@@ -220,9 +234,10 @@ class Network_Multi_Path_Infer(nn.Module):
     # ---------------------------------------------------------------------------------------------------------
     # execution
     # ---------------------------------------------------------------------------------------------------------
-    def _arm_refine(self, arm, refine, coarse, skip, out=None):
+    def _arm_refine(self, arm, refine, coarse, skip, out=None, cat=None):
         """arm 1x1 -> bilinear to skip's size -> cat([up, skip]) -> refine 3x3, with the concat done by writing both
-        producers into one buffer (model_seg.py:304-307, 309-312, 316-319)."""
+        producers into one buffer (model_seg.py:304-307, 309-312, 316-319).  cat: that buffer, its skip channels already written
+        by the skip's producer (_trunk)."""
         a = arm(coarse)
         from . import autograd as AG
         if AG.grad_mode(a):
@@ -230,9 +245,10 @@ class Network_Multi_Path_Infer(nn.Module):
             return refine(AG.cat_channels([up, skip]))
         N, c_up = a.shape[0], a.shape[1]
         c_skip, Hs, Ws = skip.shape[1], skip.shape[2], skip.shape[3]
-        cat = F_.empty_nhwc(N, c_up + c_skip, Hs, Ws, a.device)
+        if cat is None:
+            cat = F_.empty_nhwc(N, c_up + c_skip, Hs, Ws, a.device)
+            F_.copy_channels(F_.to_nhwc_half(skip), cat[:, c_up:])
         F_.bilinear(a, (Hs, Ws), out=cat[:, :c_up])
-        F_.copy_channels(F_.to_nhwc_half(skip), cat[:, c_up:])
         return refine(cat, out=out)
 
     def _side_streams(self, device):
@@ -277,8 +293,58 @@ class Network_Multi_Path_Infer(nn.Module):
         y = engine.conv_bn_act(y, stem1.conv2, stem1.bn2, relu=True)
         return self.stem[2](y)
 
+    def _fuse_resizes_for(self, input):
+        if self.fuse_resizes is False or self.training or torch.is_grad_enabled():
+            return False
+        return self.fuse_resizes or input.is_cuda
+
+    def _record_resize_plan(self, input, src_step, tap_step, shapes):
+        """The _ResizePlan of this input size, from what the first forward at that size ran: which step produced the input of each
+        step (src_step[i], None for the stem), which step's output each refine took as its skip (tap_step, the same taps the tails
+        read) and the shape of every step's output.  Buffers are then sized from the shapes the kernels produced, not re-derived
+        from each operator's stride rules."""
+        def residual(op):   # a primitive whose forward takes out_half / x_half
+            return isinstance(op, _Residual) and type(op).forward is _Residual.forward
+
+        ops = [self.cells[step.key]._op._op for step in self._steps]
+        half, reads_half = set(), set()
+        for i, p in enumerate(src_step):
+            if residual(ops[i]) and ops[i]._zoom and p is not None and residual(ops[p]):
+                half.add(p)
+                reads_half.add(i)
+        uses = {}
+        for tail in self._tails:
+            for n, (_, _, _, s_skip, _) in enumerate(self._tail_modules(tail.last)):
+                uses.setdefault(tap_step[s_skip][tail.branch], []).append((tail.branch, n))
+        skip = {p: u[0] for p, u in uses.items() if p is not None and len(u) == 1}   # a skip of two refines is copied
+        plans = self.__dict__.setdefault("_fsb_resize_plans", {})
+        plans[tuple(input.shape)] = _ResizePlan(frozenset(half), frozenset(reads_half), skip, tuple(shapes))
+
+    def _fused_outputs(self, plan, i, src_half, device, cats):
+        """keyword arguments of step i's cell under `plan`: its input's /2 (x_half), the buffer for its own /2 (out_half) and
+        its output slice of a refine's concat buffer (out, the buffer recorded in cats[(branch, link)])"""
+        kw = {}
+        if i in plan.reads_half and src_half is not None:
+            kw["x_half"] = src_half
+        N, C, Ho, Wo = plan.shapes[i]
+        if i in plan.half:
+            kw["out_half"] = F_.empty_nhwc(N, C, Ho // 2, Wo // 2, device)
+        if i in plan.skip:
+            b, n = plan.skip[i]
+            c_up = self._tail_modules(self.lasts[b])[n][0].C_out
+            cat = F_.empty_nhwc(N, c_up + C, Ho, Wo, device)
+            kw["out"] = cat[:, c_up:]
+            cats[(b, n)] = (cat, kw["out"])
+        return kw
+
     def _trunk(self, input, ctx=None):
-        """stem + cells -> per scale, the latest feature of every branch ({8: [...], 16: [...], 32: [...]})"""
+        """stem + cells -> per scale, the latest feature of every branch ({8: [...], 16: [...], 32: [...]}).
+        At inference (fuse_resizes) the kernels that produce a feature also write what later launches would have made of it:
+        - a feature that a zoomed op reads also goes out as its bilinear /2, stored by the producing kernel (the last conv of the
+          cell, or its bilinear x2 -- a /2 pixel reads only its own 2x2 block), and the zoomed op starts from that map;
+        - a refine's skip feature is written straight into the channels of the refine's concat buffer (ctx.cats).
+        Each is the same bits as the separate launch it replaces.  The first forward at an input size runs without them and
+        records the plan for that size (_record_resize_plan), like the packed-weight and folded-BN caches that it also fills."""
         full_h = input.size(2)
         ctx = ctx if ctx is not None else _BranchCtx(None)
         stem = self._stem(input)
@@ -286,20 +352,36 @@ class Network_Multi_Path_Infer(nn.Module):
         # block the caching allocator hands out cannot still be in use by main-stream work the side streams do not wait for.
         f8 = self.num_filters(8, self._stem_head_width[1])
         ctx.fused_in = F_.empty_nhwc(stem.shape[0], f8 * self._branch, stem.shape[2], stem.shape[3], stem.device)
+        fuse = self._fuse_resizes_for(input)
+        plan = self.__dict__.get("_fsb_resize_plans", {}).get(tuple(input.shape)) if fuse else None
         latest = [stem] * self._branch
+        halves = [None] * self._branch     # bilinear /2 of latest[b], where its producer wrote one
         taps = {s: [stem] * self._branch for s in SCALES}
-        for step in self._steps:
+        src_step, shapes = [], []          # what the plan is recorded from: the producer of each step's input, each output's shape
+        last_step = [None] * self._branch
+        tap_step = {s: [None] * self._branch for s in SCALES}
+        for i, step in enumerate(self._steps):
             if step.fork:
                 ctx.fork()
             with ctx.on(step.lead):
                 src = latest[step.lead]
-                feat = self.cells[step.key](src)
-                ctx.hold(src, feat)
+                # the /2 maps and concat buffers cross the branch streams like the features: allocated on the producer's stream
+                # and held until the join
+                kw = self._fused_outputs(plan, i, halves[step.lead], src.device, ctx.cats) if plan is not None else {}
+                feat = self.cells[step.key](src, **kw)
+                ctx.hold(src, feat, *kw.values())
+            src_step.append(last_step[step.lead])
+            shapes.append(tuple(feat.shape))
             stride = int(full_h // feat.size(2))
             for b in step.members:
                 latest[b] = feat
+                halves[b] = kw.get("out_half")
+                last_step[b] = i
                 if stride in taps:
                     taps[stride][b] = feat
+                    tap_step[stride][b] = i
+        if fuse and plan is None:
+            self._record_resize_plan(input, src_step, tap_step, shapes)
         return taps[8], taps[16], taps[32]
 
     def agg_ffm(self, outputs8, outputs16, outputs32, ctx=None):
@@ -328,7 +410,10 @@ class Network_Multi_Path_Infer(nn.Module):
                         aux[s_coarse].append(coarse)
                     if training and n == 1:
                         aux[s_coarse].append(taps[s_coarse][b])   # the trunk's 1/16 feature, not the refined one
-                    feat = self._arm_refine(arm, refine, coarse, taps[s_skip][b], out=slot if n == len(chain) - 1 else None)
+                    skip = taps[s_skip][b]
+                    cat, view = ctx.cats.get((b, n), (None, None))
+                    fused = {"cat": cat} if view is skip else {}   # the skip's producer wrote it into this refine's concat buffer
+                    feat = self._arm_refine(arm, refine, coarse, skip, out=slot if n == len(chain) - 1 else None, **fused)
                     ctx.hold(coarse, taps[s_skip][b], feat)
                 if not chain:
                     feat = outputs8[b]
@@ -461,6 +546,7 @@ class _BranchCtx:
         self.streams, self.forked = streams, False
         self.main = torch.cuda.current_stream() if streams else None
         self.fused_in = None
+        self.cats = {}    # (branch, link) -> (concat buffer, skip channels) a trunk cell wrote its output into
         self.keep = []
 
     def hold(self, *tensors):

@@ -241,29 +241,39 @@ class _Residual(_Primitive):
                                                                     self.dilation, self.groups))
         return latency, size_out
 
-    def forward(self, x, out=None):
+    def forward(self, x, out=None, out_half=None, x_half=None):
+        """out_half (inference): a (N, C_out, Ho // 2, Wo // 2) buffer that also receives bilinear(y, (Ho // 2, Wo // 2)), from the
+        kernel that writes y.  x_half (zoomed ops): bilinear(x, (H // 2, W // 2)) already computed, e.g. by x's producer."""
         stages = self._stages()
         if not self._zoom:
             for i, (conv, bn) in enumerate(stages):
-                x = engine.conv_bn_act(x, conv, bn, relu=True, out=out if i == len(stages) - 1 else None)
+                last = i == len(stages) - 1
+                x = engine.conv_bn_act(x, conv, bn, relu=True, out=out if last else None, out_half=out_half if last else None)
             return x
         x = F_.to_nhwc_half(x)
         H, W = int(x.size(2)), int(x.size(3))
         from . import autograd as AG
         if AG.grad_mode(x, self.conv1.weight):
+            assert out_half is None and x_half is None, "out_half / x_half are inference-only"
             y = AG.bilinear(x, (H // 2, W // 2))
             for i, (conv, bn) in enumerate(stages):
                 last = i == len(stages) - 1
                 y = engine.conv_bn_act(y, conv, bn, relu=(not last) or self.stride == 2)
             return AG.bilinear(y, (H, W), relu=True) if self.stride == 1 else y
-        y = F_.bilinear(x, (H // 2, W // 2))
+        if x_half is not None:
+            assert tuple(x_half.shape) == (x.shape[0], x.shape[1], H // 2, W // 2), (tuple(x_half.shape), tuple(x.shape))
+            y = x_half
+        else:
+            y = F_.bilinear(x, (H // 2, W // 2))
         for i, (conv, bn) in enumerate(stages):
             last = i == len(stages) - 1
             # the final ReLU comes AFTER the upsample when stride == 1 (operations.py:273-276, 442-445)
             y = engine.conv_bn_act(y, conv, bn, relu=(not last) or self.stride == 2,
-                                   out=out if (last and self.stride == 2) else None)
+                                   out=out if (last and self.stride == 2) else None,
+                                   out_half=out_half if (last and self.stride == 2) else None)
         if self.stride == 1:
-            y = F_.bilinear(y, (H, W), relu=True, out=out)
+            half = {} if out_half is None else {"out_half": out_half}
+            y = F_.bilinear(y, (H, W), relu=True, out=out, **half)
         return y
 
 

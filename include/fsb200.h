@@ -157,6 +157,14 @@ int fsb_conv_stats_rows(const fsb_conv_desc* d);
  * calculator's answer for the kernel instance and the dynamic shared memory the launcher picks.  Launches nothing.
  * FSB_ERR_UNSUPPORTED when `d` runs on the CUDA-core direct kernel; other negative values are errors. */
 int fsb_conv_residency(const fsb_conv_desc* d);
+/* fsb_conv_fwd that also writes y_half = bilinear(y, (Ho / 2, Wo / 2), align_corners=True): NHWC fp16 with pixel stride
+ * y_half_cstride (a channel slice of a wider buffer is fine), bit for bit fsb_conv_fwd followed by fsb_bilinear_fwd, in one
+ * launch (the conv tiles start on even pixels and each /2 pixel reads only its own 2x2 block).  FSB_ERR_UNSUPPORTED, before
+ * anything is written, unless the wgmma kernel runs `d` with its TMA-store epilogue (fp16 output, Cout and y_cstride multiples
+ * of 8, y 16-byte aligned), Ho and Wo are even and at most 4096, and d->flags has none of FSB_CONV_STATS, FSB_CONV_OUT_F32,
+ * FSB_CONV_Y_UP2, FSB_CONV_X_DOWN2, FSB_CONV_FORCE_DIRECT: the caller then runs the two calls. */
+int fsb_conv_fwd_half(const fsb_conv_desc* d, const void* x, const void* wpacked, const float* scale, const float* shift,
+                      void* y, void* y_half, int y_half_cstride, void* stream);
 
 /* Stem conv reading the caller's NCHW tensor directly (fp32 if x_is_f32 else fp16), 3x3 stride 2 pad 1,
  * Cin = 3, fused BN(eval)+ReLU, fp16 NHWC out.  ConvNorm at train/model_seg.py:193, search/model_search.py:148.
@@ -192,6 +200,10 @@ int fsb_confusion_matrix(int64_t n, const uint8_t* pred, const void* gt, int gt_
  * (BasicResidual_downup_*: upsample then ReLU, operations.py:275-276). */
 int fsb_bilinear_fwd(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, void* y,
                      int y_cstride, uint32_t flags, void* stream);
+/* Exact x2 upsample of fsb_bilinear_fwd (y: 2Hi x 2Wi, same flags) that also writes y_half = bilinear(y, (Hi, Wi)) (no ReLU),
+ * bit for bit the two fsb_bilinear_fwd calls, in one launch.  FSB_ERR_UNSUPPORTED when 2Hi or 2Wi exceeds 4096. */
+int fsb_bilinear_fwd_half(int N, int C, int Hi, int Wi, const void* x, int x_cstride, void* y, int y_cstride, void* y_half,
+                          int y_half_cstride, uint32_t flags, void* stream);
 /* Final logits upsample (model_seg.py:365, model_search.py:353-357): fp16 NHWC (C classes, cstride) low-res
  * logits -> NCHW output at (Ho, Wo), bilinear align_corners=True.  out_dtype: 0 = fp16, 1 = fp32. */
 int fsb_upsample_logits_nchw(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, void* y,
