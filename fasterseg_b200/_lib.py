@@ -71,6 +71,7 @@ _SIGS = {
     "fsb_upsample_logits_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_argmax": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),
     "fsb_upsample_argmax_confusion": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P, _P]),
+    "fsb_upsample_argmax_map": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P, _P, _P, _P, _P]),
     "fsb_nearest_fwd": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_logits_nearest_nchw": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, C.c_int, _P]),
     "fsb_upsample_argmax_nearest": (C.c_int, [C.c_int] * 6 + [_P, C.c_int, _P, _P]),

@@ -105,6 +105,8 @@ int bilinear_up2_half_launch(int, int, int, int, const void*, int, void*, int, v
 int upsample_logits_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
 int upsample_argmax_launch(int, int, int, int, int, int, const void*, int, uint8_t*, cudaStream_t);
 int upsample_argmax_confusion_launch(int, int, int, int, int, int, const void*, int, const void*, int, long long*, cudaStream_t);
+int upsample_argmax_map_launch(int, int, int, int, int, int, const void*, int, const uint8_t*, uint8_t*, const uint8_t*, const uint8_t*,
+                               uint8_t*, cudaStream_t);
 int train_pre_launch(const fsb_train_pre_desc&, const uint8_t*, const uint8_t*, const int32_t*, const float*, float*, long long*,
                      cudaStream_t);
 int nearest_launch(int, int, int, int, int, int, const void*, int, void*, int, cudaStream_t);
@@ -380,6 +382,12 @@ int fsb_upsample_argmax_confusion(int N, int n_cl, int Hi, int Wi, int Ho, int W
   if (N <= 0 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || !gt || !out || xcs < n_cl)
     return set_error(FSB_ERR_INVALID, "upsample_argmax_confusion: bad argument");
   return upsample_argmax_confusion_launch(N, n_cl, Hi, Wi, Ho, Wo, x, xcs, gt, gt_bytes, out, static_cast<cudaStream_t>(stream));
+}
+int fsb_upsample_argmax_map(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, const uint8_t* lut, uint8_t* ids,
+                            const uint8_t* palette, const uint8_t* image, uint8_t* viz, void* stream) {
+  if (N <= 0 || C < 1 || C > 255 || Hi <= 0 || Wi <= 0 || Ho <= 0 || Wo <= 0 || !x || xcs < C || (!ids && !viz) || (viz && !palette))
+    return set_error(FSB_ERR_INVALID, "upsample_argmax_map: bad argument");
+  return upsample_argmax_map_launch(N, C, Hi, Wi, Ho, Wo, x, xcs, lut, ids, palette, image, viz, static_cast<cudaStream_t>(stream));
 }
 int fsb_train_pre(const fsb_train_pre_desc* d, const uint8_t* img, const uint8_t* gt, const int32_t* geom, const float* lut,
                   float* out_img, int64_t* out_gt, void* stream) {

@@ -612,6 +612,91 @@ int upsample_argmax_confusion_launch(int N, int C, int Hi, int Wi, int Ho, int W
   return FSB_OK;
 }
 
+// upsample + argmax -> the two uint8 images the reference's test-set writer saves (train/test.py:49-69,
+// tools/utils/visualize.py:6-21): ids[p] = lut[label] and viz[p] = the BGR bytes of palette[label] (B, G, R, use_image), or of the
+// RGB image pixel reversed where use_image is set.  Labels are upsample_argmax4's, so they are upsample_argmax_kernel's bits.  One
+// thread = 4 consecutive output columns: one 32-bit store of ids, three of viz, where the row allows.  The tables live in shared
+// memory (C <= 255 entries).
+__global__ void __launch_bounds__(128)
+upsample_argmax_map_kernel(int N, int C, int Hi, int Wi, int Ho, int Wo, const __half* __restrict__ x, int xcs, float sh, float sw,
+                           const uint8_t* __restrict__ lut, uint8_t* __restrict__ ids, const uint8_t* __restrict__ palette,
+                           const uint8_t* __restrict__ image, uint8_t* __restrict__ viz) {
+  __shared__ uint8_t s_lut[256];
+  __shared__ uchar4 s_pal[256];
+  pdl_launch_dependents();
+  pdl_wait();
+  for (int i = threadIdx.x; i < C; i += blockDim.x) {
+    s_lut[i] = lut ? lut[i] : static_cast<uint8_t>(i);
+    if (palette) s_pal[i] = make_uchar4(palette[4 * i], palette[4 * i + 1], palette[4 * i + 2], palette[4 * i + 3]);
+  }
+  __syncthreads();
+  const int wvec = (Wo + 3) >> 2;
+  const int64_t total = static_cast<int64_t>(N) * Ho * wvec;
+  const int64_t gid = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (gid >= total) return;
+  const int wv = static_cast<int>(gid % wvec);
+  const int ho = static_cast<int>((gid / wvec) % Ho);
+  const int n = static_cast<int>(gid / (static_cast<int64_t>(wvec) * Ho));
+  int arg[4];
+  upsample_argmax4(C, Hi, Wi, Wo, x, xcs, sh, sw, n, ho, wv, arg);
+  const size_t pix = (static_cast<size_t>(n) * Ho + ho) * Wo + wv * 4;
+  const bool full = wv * 4 + 4 <= Wo;
+  if (ids) {
+    uint8_t* dst = ids + pix;
+    if (full && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
+      *reinterpret_cast<uint32_t*>(dst) = static_cast<uint32_t>(s_lut[arg[0]]) | (static_cast<uint32_t>(s_lut[arg[1]]) << 8) |
+                                          (static_cast<uint32_t>(s_lut[arg[2]]) << 16) | (static_cast<uint32_t>(s_lut[arg[3]]) << 24);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (wv * 4 + j < Wo) dst[j] = s_lut[arg[j]];
+    }
+  }
+  if (viz) {
+    uint8_t b[12];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uchar4 c = s_pal[arg[j]];
+      if (c.w && wv * 4 + j < Wo) {   // set_img_color leaves the pixel alone: the image's RGB, written reversed
+        const uint8_t* s = image + (pix + j) * 3;
+        b[3 * j] = s[2];
+        b[3 * j + 1] = s[1];
+        b[3 * j + 2] = s[0];
+      } else {
+        b[3 * j] = c.x;
+        b[3 * j + 1] = c.y;
+        b[3 * j + 2] = c.z;
+      }
+    }
+    uint8_t* dst = viz + pix * 3;
+    if (full && (reinterpret_cast<uintptr_t>(dst) & 3) == 0) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        reinterpret_cast<uint32_t*>(dst)[k] = static_cast<uint32_t>(b[4 * k]) | (static_cast<uint32_t>(b[4 * k + 1]) << 8) |
+                                              (static_cast<uint32_t>(b[4 * k + 2]) << 16) | (static_cast<uint32_t>(b[4 * k + 3]) << 24);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (wv * 4 + j < Wo) {
+          dst[3 * j] = b[3 * j];
+          dst[3 * j + 1] = b[3 * j + 1];
+          dst[3 * j + 2] = b[3 * j + 2];
+        }
+    }
+  }
+}
+
+int upsample_argmax_map_launch(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int xcs, const uint8_t* lut, uint8_t* ids,
+                               const uint8_t* palette, const uint8_t* image, uint8_t* viz, cudaStream_t stream) {
+  const int64_t total = static_cast<int64_t>(N) * Ho * ((Wo + 3) / 4);
+  const int64_t blocks = (total + 127) / 128;
+  FSB_LAUNCH(upsample_argmax_map_kernel, dim3(static_cast<unsigned>(blocks)), dim3(128), 0, stream, N, C, Hi, Wi, Ho, Wo,
+             static_cast<const __half*>(x), xcs, ac_scale(Hi, Ho), ac_scale(Wi, Wo), lut, ids, palette, image, viz);
+  cudaError_t e = last_launch_error();
+  if (e != cudaSuccess) return set_cuda_error(e, "upsample_argmax_map launch");
+  return FSB_OK;
+}
+
 // ------------------------------------------------------------------------------------------
 // nearest (latency/ deployment network): torch's legacy 'nearest' index rule, scale and product in fp32 -- for sizes like
 // 5 -> 2 or 2 -> 5 the float rounding IS the behaviour, so no integer shortcut.  Pure copies: outputs are bit-exact.

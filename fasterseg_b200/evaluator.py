@@ -41,28 +41,33 @@ def eligible(ev):
             and ev.save_path is None and not ev.show_image and not ev.show_prediction and ev.logger is None)
 
 
+def image(d):
+    """a dataset item's uint8 image as a contiguous H x W x 3 tensor (the dataset hands out a BGR->RGB flipped view)"""
+    img = d["data"]
+    if img.shape[2] < 3:                      # gray images, as process_image (tools/engine/evaluator.py:319-326) treats them
+        img = np.concatenate((img, img, img), axis=2)
+    if img.dtype != np.uint8:
+        raise TypeError("device evaluation expects the dataset's uint8 image, got %s" % img.dtype)
+    return torch.from_numpy(np.ascontiguousarray(img))
+
+
 def _collate(batch):
-    """dataset items -> (uint8 image N x H x W x 3, label N x H x W), contiguous (the dataset hands out a BGR->RGB flipped view)"""
+    """dataset items -> (uint8 image N x H x W x 3, label N x H x W), contiguous"""
     imgs, labels = [], []
     for d in batch:
-        img = d["data"]
-        if img.shape[2] < 3:                      # gray images, as process_image (tools/engine/evaluator.py:319-326) treats them
-            img = np.concatenate((img, img, img), axis=2)
-        if img.dtype != np.uint8:
-            raise TypeError("device evaluation expects the dataset's uint8 image, got %s" % img.dtype)
         lab = np.asarray(d["label"])
         if lab.dtype not in (np.uint8, np.int32, np.int64):
             lab = lab.astype(np.int64)
-        imgs.append(torch.from_numpy(np.ascontiguousarray(img)))
+        imgs.append(image(d))
         labels.append(torch.from_numpy(np.ascontiguousarray(lab)))
     return torch.stack(imgs), torch.stack(labels)
 
 
-def loader(ev):
+def loader(ev, collate_fn=_collate):
     """DataLoader over the evaluator's dataset in index order, images decoded by `ev.threds` host workers into pinned memory"""
     n = ev.ndata
     workers = max(0, min(int(ev.threds or 0), n))
-    return torch.utils.data.DataLoader(ev.dataset, batch_size=1, sampler=list(range(n)), num_workers=workers, collate_fn=_collate,
+    return torch.utils.data.DataLoader(ev.dataset, batch_size=1, sampler=list(range(n)), num_workers=workers, collate_fn=collate_fn,
                                        pin_memory=True)
 
 

@@ -450,6 +450,44 @@ def upsample_argmax_confusion(x, size, gt, n_cl, out):
     return out
 
 
+def upsample_argmax_map(x, size, lut=None, palette=None, image=None, ids_out=None, viz_out=None):
+    """The test-set writer's two images (train/test.py:49-69) from the 1/8 logits in one launch, with label = upsample_argmax(x, size):
+      ids = lut[label]                   uint8 N x Ho x Wo; written when `lut` or `ids_out` is given, or when there is no palette
+      viz = palette[label] rule          uint8 N x Ho x Wo x 3, BGR; written when `palette` is given
+    lut: uint8 [C] (None = identity).  palette: uint8 [C, 4] rows (B, G, R, use_image); where use_image is set the pixel is
+    `image`'s (uint8 N x Ho x Wo x 3, RGB) reversed to BGR, as set_img_color + `[:, :, ::-1]` (tools/utils/visualize.py:6-21) leave
+    it.  -> (ids, viz), None for an output not asked for.  Without `image` the palette's use_image column is read on the host."""
+    N, Cc, Hi, Wi, xcs = nhwc_info(x)
+    Ho, Wo = int(size[0]), int(size[1])
+    if not 1 <= Cc <= 255:
+        raise ValueError("upsample_argmax_map: 1 <= C <= 255 classes, got %d" % Cc)
+
+    def u8(t, shape, name):
+        if t.dtype != torch.uint8 or tuple(t.shape) != shape or not t.is_contiguous() or not _on_device(t) or t.device != x.device:
+            raise ValueError("upsample_argmax_map: %s must be a contiguous uint8 tensor of shape %s on %s, got %s %s on %s"
+                             % (name, shape, x.device, t.dtype, tuple(t.shape), t.device))
+        return t
+
+    if lut is not None:
+        u8(lut, (Cc,), "lut")
+    if palette is not None:
+        u8(palette, (Cc, 4), "palette")
+    elif viz_out is not None or image is not None:
+        raise ValueError("upsample_argmax_map: viz_out / image need a palette")
+    if image is not None:
+        u8(image, (N, Ho, Wo, 3), "image")
+    elif palette is not None and bool(palette[:, 3].any()):
+        raise ValueError("upsample_argmax_map: the palette takes image pixels (use_image set) but no image was given")
+    ids = viz = None
+    if ids_out is not None or lut is not None or palette is None:
+        ids = torch.empty((N, Ho, Wo), device=x.device, dtype=torch.uint8) if ids_out is None else u8(ids_out, (N, Ho, Wo), "ids_out")
+    if palette is not None:
+        viz = torch.empty((N, Ho, Wo, 3), device=x.device, dtype=torch.uint8) if viz_out is None else u8(viz_out, (N, Ho, Wo, 3), "viz_out")
+    check(_lib.lib().fsb_upsample_argmax_map(N, Cc, Hi, Wi, Ho, Wo, _ptr(x), xcs, _ptr(lut), _ptr(ids), _ptr(palette), _ptr(image),
+                                             _ptr(viz), _stream()), "fsb_upsample_argmax_map")
+    return ids, viz
+
+
 def nearest(x, size, out=None):
     """F.interpolate(x, size, mode='nearest') on NHWC fp16 views (torch's legacy index rule; a copy, so bit-exact)"""
     N, Cc, Hi, Wi, xcs = nhwc_info(x)

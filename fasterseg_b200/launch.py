@@ -265,6 +265,19 @@ def install_evaluator_patch(script):
     return finder
 
 
+def install_tester_patch(script):
+    """Test-set prediction on the device (fasterseg_b200.tester): when the driver imports the reference's engine.tester from the
+    tools/ directory next to its own (train.py:29 via train/test.py:17), patch Tester.run_online / run_online_multiprocess.
+    Returns the finder, or None (and changes nothing) when there is no such tools/engine/tester.py."""
+    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(script))), "tools", "engine", "tester.py")
+    if not os.path.isfile(path):
+        return None
+    from . import tester
+    finder = _PatchAfterImport("engine.tester", path, tester.install)
+    sys.meta_path.insert(0, finder)
+    return finder
+
+
 def install_dataloader_patch(script):
     """Training augmentation on the device (fasterseg_b200.trainpre): when the driver imports the `dataloader` module next to it
     (train/dataloader.py, search/dataloader.py), wrap its get_train_loader.  Returns the finder, or None (and changes nothing)
@@ -327,6 +340,7 @@ def main(argv=None):
     install_shadow_modules(script)
     install_data_parallel()
     install_evaluator_patch(script)
+    install_tester_patch(script)
     install_dataloader_patch(script)
     install_criterion_patch(script)
     install_train_metrics_patch(script)

@@ -490,6 +490,18 @@ class Network_Multi_Path_Infer(nn.Module):
         pred8 = self._features(input)
         cm.update_from_logits(pred8, (int(pred8.size(2)) * 8, int(pred8.size(3)) * 8), gt)
 
+    @torch.no_grad()
+    def predict_label_maps(self, input, lut=None, palette=None, ids_out=None, viz_out=None):
+        """Test-set prediction of one batch (train/test.py:49-69): the eval forward to the 1/8 logits, then one kernel upsamples,
+        takes the argmax and writes the id map lut[label] and, with a palette, the BGR colour map (functional.upsample_argmax_map).
+        A uint8 `input` (img_u8.permute(0, 3, 1, 2) after set_input_normalization) is also the image the palette's use_image rows
+        take their pixels from; a float input cannot serve them (ValueError).  -> (ids, viz)."""
+        assert not self.training
+        image = input.permute(0, 2, 3, 1) if palette is not None and input.dtype == torch.uint8 else None
+        pred8 = self._features(input)
+        return F_.upsample_argmax_map(pred8, (int(pred8.size(2)) * 8, int(pred8.size(3)) * 8), lut=lut, palette=palette, image=image,
+                                      ids_out=ids_out, viz_out=viz_out)
+
     # ---------------------------------------------------------------------------------------------------------
     # latency model (table lookups, model_seg.py:368-408)
     # ---------------------------------------------------------------------------------------------------------

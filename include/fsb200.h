@@ -218,6 +218,15 @@ int fsb_upsample_argmax(int N, int C, int Hi, int Wi, int Ho, int Wo, const void
  * map is never written.  Bit-identical counters to the two calls; 1 <= n_cl <= 64. */
 int fsb_upsample_argmax_confusion(int N, int n_cl, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, const void* gt,
                                   int gt_bytes, long long* out, void* stream);
+/* fsb_upsample_argmax fused with the test-set writer's per-pixel maps (train/test.py:49-69 after
+ * tools/engine/tester.py:179-204,270-291; colour map of tools/utils/visualize.py:6-21): with label = the fsb_upsample_argmax label,
+ *   ids[p] = lut[label]                         (lut: C entries, NULL = identity; ids [N, Ho, Wo], or NULL)
+ *   viz[p] = palette[label].use_image ? image[p] reversed to BGR : palette[label].bgr
+ * palette: C x 4 bytes (B, G, R, use_image), required with viz; image: [N, Ho, Wo, 3] RGB uint8, read only where use_image is set
+ * (the caller guarantees it is given then); viz: [N, Ho, Wo, 3] BGR, or NULL.  These are the bytes cv2.imwrite receives.
+ * 1 <= C <= 255, at least one of ids / viz. */
+int fsb_upsample_argmax_map(int N, int C, int Hi, int Wi, int Ho, int Wo, const void* x, int x_cstride, const uint8_t* lut,
+                            uint8_t* ids, const uint8_t* palette, const uint8_t* image, uint8_t* viz, void* stream);
 /* F.interpolate(mode='nearest') (torch's legacy rule, not 'nearest-exact') on fp16 NHWC channel slices (latency/ network,
  * latency/operations.py:265,269,427,434, latency/model_seg.py:305,309,315).  Per axis
  *   src = min((int)floorf((float)dst * ((float)in / (float)out)), in - 1)   in fp32, exactly as torch computes it.
